@@ -96,7 +96,10 @@ metric_reduce_kernel(const __grid_constant__ CommDev c, bool has_comm, uint64_t 
         }
     }
     if (!exchange) return;  // nothing can go wrong locally: the slot keeps whatever this reduce has recorded so far
-    if (blockIdx.x == 0 && threadIdx.x == 0) {
+    // Every CTA writes the (identical) header before its own barrier: comm_barrier only publishes the calling CTA's
+    // writes to its paired peer CTA, so a header written by CTA 0 alone could still be the one of an earlier exchange
+    // when CTA b != 0 reads it below.
+    if (threadIdx.x == 0) {
         rec_mine[0] = layout_hash;
         rec_mine[1] = (uint64_t)n_glob;
     }

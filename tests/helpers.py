@@ -86,6 +86,73 @@ def init_gloo(rank, world, initfile):
     dist.init_process_group('gloo', init_method=f'file://{initfile}', rank=rank, world_size=world)
 
 
+class Launches(list):
+    """[(kernel, grid.x)] of the dmlb:: kernels a call launched, in launch order.  `traced` is False when the profiler
+    trace held fewer dmlb:: kernels than libdmlb counted launches; the list then holds (None, None) per counted launch and
+    only its length means anything (see check_launches)."""
+    traced = True
+
+
+def check_launches(launches, expected, among=False):
+    """The witness: `launches` must be exactly `expected` (among=True: `expected` is one launch that must be among
+    them).  If the profiler lost kernel events, only the launch count is checked and a warning names the launches left
+    unwitnessed (the CPU tier still pins the grids, tests/test_launch_geometry.py).  With DMLB_WITNESS_LOG set, every
+    check is appended to that file as one JSON line."""
+    import json
+    import warnings
+
+    log = os.environ.get('DMLB_WITNESS_LOG')
+    if log:
+        with open(log, 'a') as f:
+            f.write(json.dumps({'test': os.environ.get('PYTEST_CURRENT_TEST', '').split(' ')[0], 'pid': os.getpid(),
+                                'traced': launches.traced, 'expected': expected, 'launches': list(launches)}) + '\n')
+    if launches.traced:
+        if among:
+            assert tuple(expected) in [tuple(x) for x in launches], (expected, launches)
+        else:
+            assert [tuple(x) for x in launches] == [tuple(x) for x in expected], (launches, expected)
+    else:
+        assert len(launches) >= 1 if among else len(launches) == len(expected), (len(launches), expected)
+        warnings.warn(f'profiler trace incomplete: {expected} counted, not witnessed')
+
+
+def dmlb_launches(fn):
+    """Run fn() under torch.profiler (CUDA activity) and return (fn's result, Launches) for the dmlb:: kernels it
+    launched, in launch order.  `kernel` is the demangled name without 'void ' and the parameter list, e.g.
+    'dmlb::stream_kernel<dmlb::PackF32, false>': the witness that a test size reached the launch regime it was chosen for
+    (tests/launch_geometry.py says which grid that is)."""
+    import json
+    import warnings
+
+    from torch.profiler import ProfilerActivity, profile
+
+    from dmlcloud_b200 import _native as N
+
+    torch.cuda.synchronize()
+    before = N.launch_count()
+    with profile(activities=[ProfilerActivity.CPU, ProfilerActivity.CUDA]) as prof:
+        result = fn()
+        torch.cuda.synchronize()
+    launched = N.launch_count() - before
+    with tempfile.TemporaryDirectory(prefix='dmlb_trace_') as d:
+        path = os.path.join(d, 'trace.json')
+        prof.export_chrome_trace(path)
+        with open(path) as f:
+            events = json.load(f)['traceEvents']
+    kernels = sorted((e for e in events if e.get('cat') == 'kernel' and 'dmlb::' in e.get('name', '')),
+                     key=lambda e: e['ts'])
+    out = Launches()
+    for e in kernels:
+        name = e['name']
+        name = name[len('void '):] if name.startswith('void ') else name
+        out.append((name.split('(')[0], int(e['args']['grid'][0])))
+    if len(out) != launched:
+        warnings.warn(f'the profiler trace holds {len(out)} of the {launched} libdmlb launches')
+        out = Launches([(None, None)] * launched)
+        out.traced = False
+    return result, out
+
+
 def rank_device(rank):
     """CUDA device index for a test rank: distinct GPUs when the box has several (real NVLink peers), cuda:0 shared by
     all ranks on a one-GPU box (peer mappings then go through CUDA IPC on the same device)."""

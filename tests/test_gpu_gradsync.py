@@ -13,7 +13,7 @@ import pytest
 import torch
 
 from conftest import load_npz
-from helpers import init_gloo, rank_device, spawn
+from helpers import Launches, init_gloo, rank_device, spawn
 from oracle import grad_oracle
 
 pytestmark = pytest.mark.gpu
@@ -359,3 +359,113 @@ def test_resnet18_ddp_buckets_through_the_hook_w2(wire):
         assert res['sizes'][-1] == sorted([513_000, 7_213_056, 3_963_456])  # after DDP's bucket rebuild
         # vs the fp64 mean of the per-rank gradients of an independent backward pass (cuDNN run-to-run noise included)
         assert res['worst'] <= (2e-5 if wire == 'fp32' else 1e-2), res
+
+
+# ----------------------------------------------------------------------------------------------------------------------
+# Protocol switches and grid caps of dmlb_comm_allreduce (tests/launch_geometry.py), on a 32 MB test communicator: both
+# sides of LL / one-shot and one-shot / two-shot, the first capped one-shot (forced) and two-shot, the ResNet-18 DDP bucket
+# at W = 4, and a message of exactly the communicator's capacity.  Sizes come from this device's SM count.
+# ----------------------------------------------------------------------------------------------------------------------
+BOUNDARY_MSG_BYTES = 32 << 20
+
+
+def _boundary_cases(world, sms):
+    import launch_geometry as G
+
+    cases = []  # (name, wire, algo, n)
+    for wire in ('fp32', 'bf16'):
+        sz = G.allreduce_sizes(wire == 'bf16', world, sms)
+        if world > 1:
+            cases += [(f'{wire}:ll_max', wire, 0, sz['ll_max']), (f'{wire}:ll_max_plus_1', wire, 0, sz['ll_max_plus_1'])]
+        if world == 8:
+            cases.append((f'{wire}:first_capped_twoshot', wire, 0, sz['first_capped_twoshot']))
+            continue
+        if world > 2:
+            cases += [(f'{wire}:oneshot_max', wire, 0, sz['oneshot_max']), (f'{wire}:twoshot_min', wire, 0, sz['twoshot_min']),
+                      (f'{wire}:first_capped_twoshot', wire, 0, sz['first_capped_twoshot'])]
+        cases.append((f'{wire}:first_capped_oneshot', wire, 1, sz['first_capped_oneshot']))
+    if world == 4:
+        cases.append(('fp32:resnet18_bucket', 'fp32', 0, 7_213_056))
+    if world in (2, 4):
+        cases.append(('fp32:at_msg_cap', 'fp32', 0, BOUNDARY_MSG_BYTES // 4))
+    return cases
+
+
+def _allreduce_boundary_worker(rank, world, initfile, outdir):
+    init_gloo(rank, world, initfile)
+    import hashlib
+
+    import torch.distributed as dist
+
+    import launch_geometry as G
+    from dmlcloud_b200 import _native as N
+    from dmlcloud_b200.gradsync import WIRES, PeerComm
+    from helpers import dmlb_launches
+
+    di = rank_device(rank)
+    torch.cuda.set_device(di)
+    dev = torch.device('cuda', di)
+    sms = N.device_info(di)['sm_count']
+    lib, st = N.cuda_lib(di), N.stream_ptr()
+    comm = PeerComm(dev, None, max_message_bytes=BOUNDARY_MSG_BYTES)
+    sumsq = torch.zeros(1, dtype=torch.float64, device=dev)
+    results = {}
+    for name, wire, algo, n in _boundary_cases(world, sms):
+        locals_ = np.stack([np.random.RandomState(7919 * r + n % 7919).randn(n).astype(np.float32) * 3 for r in range(world)])
+        buf = torch.from_numpy(locals_[rank]).to(dev)
+        sumsq.zero_()
+
+        def call():
+            return lib.dmlb_comm_allreduce(comm.handle, buf.data_ptr(), n, WIRES[wire], 1.0 / world, sumsq.data_ptr(),
+                                           algo, None, st)
+
+        rc, launches = dmlb_launches(call)
+        N.check(rc, name)
+        proto, grid, _ = G.allreduce_plan(n, wire == 'bf16', world, sms, algo=algo)
+        got = buf.cpu().numpy()
+        want = grad_oracle.allreduce_f32(locals_) if wire == 'fp32' else \
+            grad_oracle.allreduce_bf16(locals_, round_result=proto == 'twoshot')
+        sq = float(np.sum(got.astype(np.float64) ** 2))
+        results[name] = {'proto': proto, 'grid': grid, 'traced': launches.traced, 'launches': list(launches),
+                         'bit_exact': bool((got.view(np.uint32) == want.view(np.uint32)).all()),
+                         'sumsq_rel': abs(sumsq.item() - sq) / max(sq, 1e-300),
+                         'digest': hashlib.sha256(got.tobytes()).hexdigest()}
+    if world > 1:  # one vector more than the arena's message capacity: refused before any launch
+        big = torch.zeros(BOUNDARY_MSG_BYTES // 4 + 4, device=dev)
+        before = N.launch_count()
+        rc = lib.dmlb_comm_allreduce(comm.handle, big.data_ptr(), BOUNDARY_MSG_BYTES // 4 + 1, WIRES['fp32'], 1.0, None, 0,
+                                     None, st)
+        results['over_msg_cap'] = {'rc': rc, 'launches': N.launch_count() - before}
+    Path(outdir, f'r{rank}.json').write_text(json.dumps(results))
+    dist.barrier()
+    comm.close()
+    dist.destroy_process_group()
+
+
+@pytest.mark.parametrize('world', [1, 2, 3, 4, 8])
+def test_allreduce_at_protocol_switches_and_grid_caps(world):
+    from dmlcloud_b200 import _native as N
+    from helpers import check_launches
+
+    out = spawn(_allreduce_boundary_worker, world, timeout=900)
+    res = [json.loads((out / f'r{r}.json').read_text()) for r in range(world)]
+    for name, e in res[0].items():
+        if name == 'over_msg_cap':
+            for r in range(world):
+                assert res[r][name] == {'rc': N.ECAPACITY, 'launches': 0}, (r, res[r][name])
+            continue
+        for r in range(world):
+            f = res[r][name]
+            assert f['bit_exact'] and f['sumsq_rel'] < 1e-12, (name, r, f)
+            assert f['digest'] == e['digest'], (name, r)  # bit-identical on every rank
+            launches = Launches([tuple(x) for x in f['launches']])
+            launches.traced = f['traced']
+            (kernel, grid), = launches if f['traced'] else [(None, None)]
+            if f['traced']:
+                assert kernel.startswith(f'dmlb::allreduce_{f["proto"]}_kernel<'), (name, kernel)
+            check_launches(launches, [(kernel, f['grid'])])
+    names = set(res[0])
+    if world > 2 and world != 8:
+        assert res[0][f'fp32:oneshot_max']['proto'] == 'oneshot' and res[0]['fp32:twoshot_min']['proto'] == 'twoshot'
+    if world > 1:
+        assert res[0]['fp32:ll_max']['proto'] == 'll' and res[0]['fp32:ll_max_plus_1']['proto'] != 'll', names

@@ -199,6 +199,140 @@ class TestBucketKernels:
         assert (out1.cpu().numpy()[idx] == want).all()
 
 
+def _sms():
+    return N_().device_info(0)['sm_count']
+
+
+STREAM_ENTRIES = ['scale', 'pack_f32', 'pack_bf16', 'unpack_bf16_sumsq', 'round_bf16_sumsq', 'sumsq', 'clip']
+STREAM_FUNCTOR = {'scale': 'ScaleInplace', 'pack_f32': 'PackF32', 'pack_bf16': 'PackBf16',
+                  'unpack_bf16_sumsq': 'UnpackBf16<true>', 'round_bf16_sumsq': 'RoundBf16Inplace<true>',
+                  'sumsq': 'SumsqF32', 'clip': 'ClipF32'}
+STREAM_REGIMES = ['last_first_wave', 'first_rounded_grid', 'last_chunked', 'first_grid_stride', 'grid_stride_head']
+
+
+def _f64_sumsq(x):
+    return float(np.sum(np.asarray(x, dtype=np.float64) ** 2))
+
+
+def _run_stream_entry(lib, entry, n, off, seed):
+    """One launch_stream entry point on n elements starting `off` elements into a 16-byte aligned allocation (so the
+    kernel's scalar head is (4 - off) % 4 elements).  Returns (got, want, sumsq got, sumsq want, launches)."""
+    from helpers import check_launches, dmlb_launches
+
+    N = N_()
+    g = rand_grads(n + 8, seed)
+    gv = g[off:off + n]
+    st = sptr()
+    sumsq = torch.zeros(1, dtype=torch.float64, device='cuda')
+    want_sq = None
+    if entry in ('scale', 'round_bf16_sumsq', 'sumsq', 'clip'):
+        x = torch.from_numpy(g).cuda()[off:off + n]
+        if entry == 'scale':
+            call = lambda: lib.dmlb_bucket_scale_f32(x.data_ptr(), n, 0.125, st)
+            want = grad_oracle.scale_f32(gv, 8)
+        elif entry == 'round_bf16_sumsq':
+            call = lambda: lib.dmlb_bucket_round_bf16_f32(x.data_ptr(), n, 0.25, sumsq.data_ptr(), st)
+            want = grad_oracle.round_bf16(grad_oracle.scale_f32(gv, 4))
+            want_sq = _f64_sumsq(want)
+        elif entry == 'sumsq':
+            call = lambda: lib.dmlb_bucket_sumsq_f32(x.data_ptr(), n, sumsq.data_ptr(), st)
+            want, want_sq = gv, _f64_sumsq(gv)
+        else:  # clip: the coefficient is formed on the device from the fp64 sum, in fp32 like clip_grad_norm_
+            sq = _f64_sumsq(gv)
+            sumsq.fill_(sq)
+            total = np.float32(np.sqrt(sq))
+            coef = min(np.float32(1.0), np.float32(np.float32(1.5) / np.float32(total + np.float32(1e-6))))
+            call = lambda: lib.dmlb_bucket_clip_f32(x.data_ptr(), n, sumsq.data_ptr(), 1.5, st)
+            want = (gv * np.float32(coef)).astype(np.float32)
+        out = x
+    elif entry == 'pack_f32':
+        x = torch.from_numpy(g).cuda()[off:off + n]
+        out = torch.zeros(n + 8, device='cuda')[off:off + n]
+        call = lambda: lib.dmlb_bucket_pack_f32_f32(x.data_ptr(), out.data_ptr(), n, 0.125, st)
+        want = grad_oracle.scale_f32(gv, 8)
+    elif entry == 'pack_bf16':
+        x = torch.from_numpy(g).cuda()[off:off + n]
+        wire = torch.zeros(n + 8, dtype=torch.bfloat16, device='cuda')
+        out = wire[off:off + n]
+        call = lambda: lib.dmlb_bucket_pack_f32_bf16(x.data_ptr(), out.data_ptr(), n, 0.125, st)
+        want = grad_oracle.round_bf16(grad_oracle.scale_f32(gv, 8))
+    else:  # unpack_bf16_sumsq
+        bits = grad_oracle.f32_to_bf16_bits(g)
+        src = torch.from_numpy(bits.view(np.int16)).cuda().view(torch.bfloat16)[off:off + n]
+        out = torch.full((n + 8,), -7.0, device='cuda')[off:off + n]
+        call = lambda: lib.dmlb_bucket_unpack_bf16_f32(src.data_ptr(), out.data_ptr(), n, 2.0, sumsq.data_ptr(), st)
+        want = grad_oracle.bf16_bits_to_f32(bits[off:off + n]) * np.float32(2.0)
+        want_sq = _f64_sumsq(want)
+    rc, launches = dmlb_launches(call)
+    N.check(rc, entry)
+    got = out.float().cpu().numpy() if entry != 'sumsq' else gv
+    return got, want, sumsq.item(), want_sq, launches
+
+
+class TestBucketKernelBoundaries:
+    """Every launch_stream entry point at the edges of its launch regimes on this device (tests/launch_geometry.py):
+    the last one-CTA-per-SM grid, the first grid rounded up to a multiple of the SM count, the last two-wave chunked
+    launch, the first grid-stride launch and a grid-stride launch with an unaligned scalar head."""
+
+    @pytest.mark.parametrize('regime', STREAM_REGIMES)
+    @pytest.mark.parametrize('entry', STREAM_ENTRIES)
+    def test_stream_entry_at_regime_edge(self, lib, entry, regime):
+        import launch_geometry as G
+        from helpers import check_launches
+
+        sms = _sms()
+        sizes = G.stream_sizes(sms)
+        if regime == 'grid_stride_head':
+            n, off = sizes['first_grid_stride'] + 4097, 1 + STREAM_ENTRIES.index(entry) % 3
+        else:
+            n, off = sizes[regime], 0
+        head = (4 - off) % 4
+        grid, chunk = G.launch_stream(n, head, sms)
+        assert (chunk == 0) == (regime in ('first_grid_stride', 'grid_stride_head'))
+        got, want, sq, want_sq, launches = _run_stream_entry(lib, entry, n, off, 1000 + n + off)
+        check_launches(launches, [(f'dmlb::stream_kernel<dmlb::{STREAM_FUNCTOR[entry]}, {"true" if want_sq else "false"}>',
+                                   grid)])
+        assert (got.view(np.uint32) == want.view(np.uint32)).all(), int((got != want).sum())
+        if want_sq is not None:
+            np.testing.assert_allclose(sq, want_sq, rtol=1e-12)
+
+    @pytest.mark.parametrize('case', ['regs_below_tma', 'tma', 'tma_plus_tail', 'tma_size_misaligned'])
+    def test_bf16_dispatcher_hands_over_to_tma(self, lib, case):
+        """dmlb_bucket_pack_f32_bf16 / unpack_bf16_f32 take the TMA kernels from kTmaMinElems on when both pointers are
+        16-byte aligned, the register kernels otherwise; a ragged tail after the TMA body is one more launch."""
+        import launch_geometry as G
+        from helpers import check_launches, dmlb_launches
+
+        N = N_()
+        n = {'regs_below_tma': G.K_TMA_MIN_ELEMS - 1, 'tma': G.K_TMA_MIN_ELEMS, 'tma_plus_tail': G.K_TMA_MIN_ELEMS + 5,
+             'tma_size_misaligned': G.K_TMA_MIN_ELEMS}[case]
+        off = 1 if case == 'tma_size_misaligned' else 0
+        g = torch.randn(n + 8, device='cuda')
+        src = g[off:off + n]
+        wire = torch.zeros(n + 8, dtype=torch.bfloat16, device='cuda')[off:off + n]
+        out = torch.full((n + 8,), -3.0, device='cuda')[off:off + n]
+        st = sptr()
+
+        def both():
+            N.check(lib.dmlb_bucket_pack_f32_bf16(src.data_ptr(), wire.data_ptr(), n, 0.125, st))
+            N.check(lib.dmlb_bucket_unpack_bf16_f32(wire.data_ptr(), out.data_ptr(), n, 2.0, None, st))
+
+        _, launches = dmlb_launches(both)
+        regs = ['dmlb::stream_kernel<dmlb::PackBf16, false>', 'dmlb::stream_kernel<dmlb::UnpackBf16<false>, false>']
+        want_names = {'regs_below_tma': regs, 'tma_size_misaligned': regs,
+                      'tma': ['dmlb::pack_bf16_tma_kernel', 'dmlb::unpack_bf16_tma_kernel'],
+                      'tma_plus_tail': ['dmlb::pack_bf16_tma_kernel', regs[0], 'dmlb::unpack_bf16_tma_kernel', regs[1]]}
+        if case in ('regs_below_tma', 'tma_size_misaligned'):  # the register path: grids as launch_stream picks them
+            grid = G.launch_stream(n, (4 - off) % 4, _sms())[0]
+            check_launches(launches, [(regs[0], grid), (regs[1], grid)])
+        else:  # TMA: its grid is not restated; the kernel sequence is the witness
+            check_launches(launches, [(k, g) for k, (_, g) in zip(want_names[case], launches)])
+        gv = src.cpu().numpy()
+        want = grad_oracle.round_bf16(grad_oracle.scale_f32(gv, 8))
+        assert (wire.float().cpu().numpy() == want).all()
+        assert (out.cpu().numpy() == want * np.float32(2.0)).all()
+
+
 class TestShardKernels:
     def test_gather_normalise_matches_torchvision_arithmetic(self, lib):
         N = N_()
@@ -251,3 +385,26 @@ class TestShardKernels:
         ds = DeviceShardedDataset(images[:1000], labels[:1000], batch_size=50, shuffle=True, seed=case['seed'],
                                   rank=2, world_size=case['world'], device='cuda:0')
         assert torch.cat([y for _, y in ds]).cpu().tolist() == case['out']  # epoch 0 -> the reference's own list
+
+    @pytest.mark.parametrize('out_bf16', [0, 1], ids=['fp32', 'bf16'])
+    def test_gather_at_capped_grid(self, lib, out_bf16):
+        """A batch of 8,192 MNIST images: more 16-pixel vectors than the grid (capped at 8 CTAs per SM) has threads, so
+        every thread walks several of them."""
+        import launch_geometry as G
+        from helpers import check_launches, dmlb_launches
+
+        N = N_()
+        batch, row = 8192, 784
+        rng = np.random.RandomState(4)
+        images = torch.from_numpy(rng.randint(0, 256, (10000, row)).astype(np.uint8)).cuda()
+        idx = torch.from_numpy(rng.randint(0, 10000, batch)).cuda()
+        dt = torch.bfloat16 if out_bf16 else torch.float32
+        x = torch.empty(batch, row, dtype=dt, device='cuda')
+        rc, launches = dmlb_launches(lambda: lib.dmlb_shard_gather_u8(images.data_ptr(), idx.data_ptr(), batch, row, 0.1307,
+                                                                      0.3081, x.data_ptr(), out_bf16, sptr()))
+        N.check(rc)
+        grid = G.shard_grid(batch * row // 16, _sms())
+        check_launches(launches, [(f'dmlb::shard_gather_u8_kernel<{"true" if out_bf16 else "false"}>', grid)])
+        assert grid * 256 < batch * row // 16
+        want = images[idx].cpu().float().div(255).sub(0.1307).div(0.3081)
+        assert torch.equal(x.cpu(), want.to(dt))

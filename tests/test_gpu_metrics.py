@@ -390,3 +390,253 @@ class TestSlabEdgeCases:
         assert combine(full, full) == N.METRIC_SPLIT_VOTE  # sticky until the caller clears the block
         out[:STATUS_BYTES].zero_()
         assert combine(full, full) == N.METRIC_OK
+
+
+# ----------------------------------------------------------------------------------------------------------------------
+# Launch-regime edges of the metric kernels (tests/launch_geometry.py): the warp path of fold_entry, the exchanging reduce
+# whose CTAs loop over more than one pass of global cells, the reset grid capped at the SM count, and the header check of
+# the exchanging reduce under alternating layouts.
+# ----------------------------------------------------------------------------------------------------------------------
+FOLD_DTYPES = [torch.float32, torch.float64, torch.float16, torch.bfloat16, torch.int64, torch.int32, torch.uint8]
+
+
+def _fold_values(dtype, shape, rng):
+    if dtype == torch.int64:  # sums beyond 2**53 (fp64 could not hold them), far below 2**63
+        v = rng.randint(2 ** 49, 2 ** 50, shape, dtype=np.int64) * rng.choice([-1, 1, 1], shape)
+    elif dtype == torch.int32:
+        v = rng.randint(-2 ** 31, 2 ** 31 - 1, shape, dtype=np.int64)
+    elif dtype == torch.uint8:
+        v = rng.randint(0, 256, shape)
+    else:
+        v = rng.randn(*shape) * 10.0 ** rng.randint(-3, 4, shape)
+    return torch.tensor(v).to(dtype)
+
+
+@pytest.mark.parametrize('dtype', FOLD_DTYPES, ids=lambda d: str(d).replace('torch.', ''))
+def test_fold_warp_path_every_shape_against_fsum(dtype):
+    """dmlb_metric_fold + dmlb_metric_reduce (W = 1) with k in {31, 32, 33, 1000}, lanes in {1, 3}, steps in {1, 3} and
+    every op: steps * k >= 32 takes the warp path, whose element index is st * (lanes * k) + lane * k + j.  Float cells
+    carry the fp64 descriptor bit, so the raw fp64 accumulation comes back; integers and MIN / MAX must be exact (a NaN
+    sits at an element warp lane 0 never loads), float sums within per_cell * 2**-52 * sum|x| of math.fsum."""
+    import math
+
+    from dmlcloud_b200 import _native as N
+    from dmlcloud_b200.metrics import STATUS_BYTES
+    from helpers import check_launches, dmlb_launches
+
+    lib, st = N.cuda_lib(0), N.stream_ptr()
+    is_int = not dtype.is_floating_point
+    ops = [N.SUM, N.MIN, N.MAX] if is_int else [N.MEAN, N.SUM, N.MIN, N.MAX]
+    rng = np.random.RandomState(FOLD_DTYPES.index(dtype))
+    cases, cell = [], 0
+    for k in (31, 32, 33, 1000):
+        for lanes in (1, 3):
+            for steps in (1, 3):
+                for op in ops:
+                    x = _fold_values(dtype, (steps, lanes, k), rng)
+                    if op in (N.MIN, N.MAX) and not is_int and steps * k >= 33:
+                        x.view(steps, lanes * k)[0, (lanes - 1) * k + 1] = float('nan')  # element t = 1 of the last lane
+                    cases.append((cell, k, lanes, steps, op, x))
+                    cell += lanes
+    C = cell
+    desc = torch.tensor([0] * C, dtype=torch.int32)
+    for c0, k, lanes, steps, op, _ in cases:
+        desc[c0:c0 + lanes] = op | (int(is_int) << 2) | (int(not is_int) << 4)
+    desc = desc.cuda()
+    acc = torch.zeros(C, dtype=torch.int64, device='cuda')
+    cnt = torch.zeros(C, dtype=torch.int64, device='cuda')
+    out = torch.zeros(STATUS_BYTES + 9 * C, dtype=torch.uint8, device='cuda')
+    srcs = [x.cuda().contiguous() for *_, x in cases]
+    entries = [N.FoldEntry(s.data_ptr(), 0, {torch.float32: N.F32, torch.float64: N.F64, torch.float16: N.F16,
+                                             torch.bfloat16: N.BF16, torch.int64: N.I64, torch.int32: N.I32,
+                                             torch.uint8: N.U8}[dtype], c0, lanes, k, steps, 0)
+               for s, (c0, k, lanes, steps, op, _) in zip(srcs, cases)]
+    ranges = (N.Range * 1)(N.Range(0, C))
+    base = out.data_ptr()
+
+    def run():
+        N.check(lib.dmlb_metric_reset(acc.data_ptr(), cnt.data_ptr(), desc.data_ptr(), 0, C, st))
+        for i in range(0, len(entries), N.MAX_FOLD_ENTRIES):
+            part = entries[i:i + N.MAX_FOLD_ENTRIES]
+            N.check(lib.dmlb_metric_fold(acc.data_ptr(), cnt.data_ptr(), desc.data_ptr(),
+                                         (N.FoldEntry * len(part))(*part), len(part), st))
+        N.check(lib.dmlb_metric_reduce(None, acc.data_ptr(), cnt.data_ptr(), desc.data_ptr(), C, ranges, 1, 0, 0, 1,
+                                       base + STATUS_BYTES, base + STATUS_BYTES + 8 * C, base, st))
+
+    _, launches = dmlb_launches(run)
+    folds = [min(N.MAX_FOLD_ENTRIES, len(entries) - i) for i in range(0, len(entries), N.MAX_FOLD_ENTRIES)]
+    check_launches(launches, [('dmlb::metric_reset_kernel', -(-C // 256))] + [('dmlb::metric_fold_kernel', f) for f in folds]
+                   + [('dmlb::metric_reduce_kernel', -(-C // 256))])
+    host = out.cpu()
+    assert int(host[:STATUS_BYTES].view(torch.int32).abs().max()) == N.METRIC_OK
+    vals = host[STATUS_BYTES:STATUS_BYTES + 8 * C].view(torch.int64 if is_int else torch.float64).numpy()
+    flags = host[STATUS_BYTES + 8 * C:].numpy()
+    assert (flags == 0).all()
+    for c0, k, lanes, steps, op, x in cases:
+        xs = x.to(torch.int64 if is_int else torch.float64).numpy()  # exact: every source dtype widens exactly
+        for lane in range(lanes):
+            e = xs[:, lane, :].ravel()
+            got = vals[c0 + lane]
+            what = (str(dtype), k, lanes, steps, op, lane)
+            if op == N.MIN or op == N.MAX:
+                f = np.min if op == N.MIN else np.max
+                want = f(e)  # numpy min / max propagate NaN like torch.amin / amax
+                assert (np.isnan(got) and np.isnan(want)) if not is_int and np.isnan(want) else got == want, (what, got, want)
+            elif is_int:
+                assert int(got) == sum(int(v) for v in e), what
+            else:
+                exact = math.fsum(e.tolist())
+                tol = len(e) * 2.0 ** -52 * float(np.abs(e).sum())
+                want = exact / len(e) if op == N.MEAN else exact
+                assert abs(got - want) <= (tol / len(e) if op == N.MEAN else tol) + 1e-300, (what, got, want)
+
+
+def test_min_metric_wider_than_the_reset_grid_over_two_epochs():
+    """A MIN metric with more lanes than one pass of the SM-count-capped reset grid covers.  The first epoch exercises
+    metric_reset_kernel: registering the metric resets its freshly zeroed cells to +inf, and a lane it missed would keep
+    0.0, below every tracked value (>= 5).  The second epoch exercises the reset the epoch-closing reduce does itself
+    (finalize_cell): it must not see the first epoch's values."""
+    import launch_geometry as G
+    from dmlcloud_b200 import _native as N
+    from dmlcloud_b200.metrics import MetricTracker, Reduction
+    from helpers import check_launches, dmlb_launches
+
+    sms = N.device_info(0)['sm_count']
+    lanes = G.metric_sizes(sms)['reset_first_capped'] + 6207  # 40,000 on 132 SMs
+    t = MetricTracker()
+    t.register_metric('m', Reduction.MIN, dim=[0])
+    first = torch.rand(2, lanes, device='cuda') + 5.0
+    second = torch.rand(2, lanes, device='cuda') + 7.0
+    _, launches = dmlb_launches(lambda: t.track('m', first))
+    check_launches(launches, ('dmlb::metric_reset_kernel', G.metric_reset_grid(lanes, sms)), among=True)
+    assert G.metric_reset_grid(lanes, sms) * 256 < lanes
+    t.next_epoch()
+    t.track('m', second)
+    t.next_epoch()
+    assert torch.equal(t['m'][0], first.amin(0).cpu())
+    assert torch.equal(t['m'][1], second.amin(0).cpu())
+
+
+def _exchange_many_cells_worker(rank, world, initfile, outdir):
+    """> 2048 global cells in 40 ranges plus 40 one-cell rank-local ranges, through the peer exchange, against the numpy
+    slab oracle replaying the same session (bit-exact)."""
+    init_gloo(rank, world, initfile)
+    import torch.distributed as dist
+
+    import launch_geometry as G
+    from dmlcloud_b200 import _native as N
+    from dmlcloud_b200.gradsync import PeerComm
+    from dmlcloud_b200.metrics import MetricTracker, Reduction
+    from helpers import assert_histories_match, check_launches, dmlb_launches, rank_device
+    from oracle.slab_oracle import OracleSlab
+
+    torch.cuda.set_device(rank_device(rank))
+    dev = torch.device('cuda', rank_device(rank))
+    comm = PeerComm(dev, None, max_message_bytes=1 << 20)
+    t = MetricTracker()
+    t.bind(device=dev, comm=comm, group=None)
+    o = MetricTracker()
+    o.bind(slab=OracleSlab())
+    ops = [Reduction.MEAN, Reduction.SUM, Reduction.MIN, Reduction.MAX]
+    n_glob = G.metric_sizes(N.device_info(dev.index)['sm_count'])['exchange_first_looping'] + 351  # 2,400
+    per_block = n_glob // 40
+    for tr in (t, o):
+        for b in range(40):
+            for i in range(per_block):
+                tr.register_metric(f'g{b}_{i}', ops[(b + i) % 4])
+            tr.register_metric(f'loc{b}', Reduction.SUM, globally=False)
+    names = [f'g{b}_{i}' for b in range(40) for i in range(per_block)] + [f'loc{b}' for b in range(40)]
+    rng = np.random.RandomState(rank)
+    for step in range(2):
+        vals = rng.randn(len(names)).astype(np.float32)
+        for name, v in zip(names, vals.tolist()):
+            t.track(name, v)
+            o.track(name, v)
+    t._slab.flush_all()
+    if rank == 0:
+        _, launches = dmlb_launches(t.next_epoch)
+        check_launches(launches, ('dmlb::metric_reduce_kernel', G.K_EXCHANGE_GRID), among=True)
+    else:
+        t.next_epoch()
+    o.next_epoch()
+    assert_histories_match(t.histories, t.epoch,
+                           {'epoch': o.epoch, 'histories': {k: [_enc(v) for v in h] for k, h in o.histories.items()}},
+                           exact_float=True)
+    Path(outdir, f'ok{rank}').write_text('ok')
+    dist.barrier()
+    comm.close()
+    dist.destroy_process_group()
+
+
+@pytest.mark.parametrize('world', [2, 4])
+def test_exchanging_reduce_loops_over_more_than_one_pass_of_cells(world):
+    out = spawn(_exchange_many_cells_worker, world, timeout=600)
+    assert all((out / f'ok{r}').exists() for r in range(world))
+
+
+def _alternating_layout_worker(rank, world, initfile, outdir, n_iter):
+    """A fresh metric communicator, then n_iter exchanging reduces through the C ABI cycling through three layouts with
+    different hashes and cell counts (1-3 global cells, so CTAs 1-7 of the reduce own no cells and reach the header check
+    at once).  Values are folded between reduces; every call must return METRIC_OK and the rank-ordered sum."""
+    init_gloo(rank, world, initfile)
+    import torch.distributed as dist
+
+    from dmlcloud_b200 import _native as N
+    from dmlcloud_b200.gradsync import PeerComm
+    from dmlcloud_b200.metrics import STATUS_BYTES
+    from helpers import check_launches, dmlb_launches, rank_device
+
+    torch.cuda.set_device(rank_device(rank))
+    dev = torch.device('cuda', rank_device(rank))
+    lib, st = N.cuda_lib(dev.index), N.stream_ptr()
+    comm = PeerComm(dev, None, max_message_bytes=1 << 16)
+    C = 3
+    desc = torch.full((C,), N.SUM | (1 << 3) | (1 << 4), dtype=torch.int32, device=dev)  # global fp64 SUM
+    acc = torch.zeros(C, dtype=torch.int64, device=dev)
+    cnt = torch.zeros(C, dtype=torch.int64, device=dev)
+    N.check(lib.dmlb_metric_reset(acc.data_ptr(), cnt.data_ptr(), desc.data_ptr(), 0, C, st))
+    row = -(-(STATUS_BYTES + 9 * C) // 256) * 256  # every result block 256-byte aligned (values are u64, status i32)
+    out = torch.zeros(n_iter + 1, row, dtype=torch.uint8, device=dev)
+    layouts = [(1, 0x1111), (2, 0x2222_0000_0002), (3, 0x3333_0000_0000_0003)]
+    import struct
+
+    def one(i):
+        n, h = layouts[i % 3]
+        v = float((rank + 1) * (i + 1))
+        bits = struct.unpack('<q', struct.pack('<d', v))[0]
+        ent = (N.FoldEntry * n)(*[N.FoldEntry(None, bits, N.F64, c, 1, 1, 1, 0) for c in range(n)])
+        N.check(lib.dmlb_metric_fold(acc.data_ptr(), cnt.data_ptr(), desc.data_ptr(), ent, n, st))
+        base = out[i].data_ptr()
+        rng = (N.Range * 1)(N.Range(0, n))
+        N.check(lib.dmlb_metric_reduce(comm.handle, acc.data_ptr(), cnt.data_ptr(), desc.data_ptr(), C, rng, 1, 1, h, 1,
+                                       base + STATUS_BYTES, base + STATUS_BYTES + 8 * C, base, st))
+
+    for i in range(n_iter):
+        one(i)
+    if rank == 0:
+        _, launches = dmlb_launches(lambda: one(n_iter))
+        check_launches(launches, [('dmlb::metric_fold_kernel', layouts[n_iter % 3][0]), ('dmlb::metric_reduce_kernel', 8)])
+    else:
+        one(n_iter)
+    torch.cuda.synchronize()
+    host = out.cpu()
+    bad = []
+    for i in range(n_iter + 1):
+        n = layouts[i % 3][0]
+        status = int(host[i, :STATUS_BYTES].view(torch.int32).max())
+        vals = host[i, STATUS_BYTES:STATUS_BYTES + 8 * C].view(torch.float64)[:n].tolist()
+        want = float(sum((r + 1) * (i + 1) for r in range(world)))
+        if status != N.METRIC_OK or vals != [want] * n:
+            bad.append((i, status, vals))
+    Path(outdir, f'r{rank}').write_text(json.dumps(bad))
+    dist.barrier()
+    comm.close()
+    dist.destroy_process_group()
+
+
+@pytest.mark.parametrize('world', [2, 4])
+def test_exchanging_reduce_header_check_under_alternating_layouts(world):
+    out = spawn(_alternating_layout_worker, world, 200, timeout=600)
+    for r in range(world):
+        bad = json.loads((out / f'r{r}').read_text())
+        assert not bad, (r, len(bad), bad[:5])

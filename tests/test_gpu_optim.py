@@ -290,3 +290,119 @@ def test_flat_sgd_matches_torch_sgd_and_follows_a_scheduler():
     for i, p in enumerate(a.parameters()):
         torch.testing.assert_close(other.state_dict()['state'][i]['momentum_buffer'], ref.state[p]['momentum_buffer'],
                                    rtol=1e-5, atol=1e-6)
+
+
+# ----------------------------------------------------------------------------------------------------------------------
+# Sizes past one grid sweep (tests/launch_geometry.py): the first size whose vector path needs a second sweep of the
+# capped grid, and ResNet-18's 11,689,512 parameters (11 sweeps on 132 SMs); vector and shifted scalar path.
+# ----------------------------------------------------------------------------------------------------------------------
+def _sweep_size(regime):
+    import launch_geometry as G
+    from dmlcloud_b200 import _native as N
+
+    return G.optim_sizes(N.device_info(0)['sm_count'])['first_multi_sweep'] if regime == 'first_multi_sweep' else 11_689_512
+
+
+def _witness_first_launch(call, kernel, n, shift):
+    """Run call() (one optimizer launch) under the profiler; assert it is `kernel`<4|1> on the grid launch_geometry
+    predicts for this device, and that this grid needs more than one sweep."""
+    import launch_geometry as G
+    from dmlcloud_b200 import _native as N
+    from helpers import check_launches, dmlb_launches
+
+    sms = N.device_info(0)['sm_count']
+    rc, launches = dmlb_launches(call)
+    N.check(rc, kernel)
+    vector = shift == 0
+    check_launches(launches, [(f'dmlb::{kernel}<{4 if vector else 1}>', G.optim_grid(n, vector, sms))])
+    assert G.optim_sweeps(n, vector, sms) > 1
+
+
+@pytest.mark.parametrize('shift', [0, 1], ids=['vector', 'shifted_scalar'])
+@pytest.mark.parametrize('regime', ['first_multi_sweep', 'resnet18_params'])
+@pytest.mark.parametrize('cfg', [1, 2], ids=['adam_l2', 'adamw_maximize'])
+def test_adam_kernel_past_one_sweep(regime, shift, cfg):
+    """4 steps: two with the host learning rate, then two reading it from device memory (the host value passed is
+    garbage; AdamW's decay factor must be recomputed from the device lr), the last one also zeroing the gradient."""
+    from dmlcloud_b200 import _native as N
+
+    c = CONFIGS[cfg]
+    n = _sweep_size(regime)
+    lib, st = N.cuda_lib(0), N.stream_ptr()
+    rng = np.random.RandomState(n % 1000 + 10 * cfg + shift)
+    P = rng.randn(n).astype(np.float32)
+    Pd, M, V = P.astype(np.float64), np.zeros(n), np.zeros(n)
+    dev = [torch.zeros(n + shift, dtype=torch.float32, device='cuda') for _ in range(4)]
+    p, g, m, v = (t[shift:] for t in dev)
+    p.copy_(torch.from_numpy(P))
+    state = torch.zeros(2, dtype=torch.int64, device='cuda')
+    lr_t = torch.full((1,), c['lr'], dtype=torch.float64, device='cuda')
+    for t in range(1, 5):
+        G = (rng.randn(n) * (0.05 if t % 2 else 4.0)).astype(np.float32)
+        g.copy_(torch.from_numpy(G))
+        on_dev = t >= 3
+
+        def call():
+            return lib.dmlb_adam_step_f32(p.data_ptr(), g.data_ptr(), m.data_ptr(), v.data_ptr(), n,
+                                          123.0 if on_dev else c['lr'], c['betas'][0], c['betas'][1], c['eps'],
+                                          c['weight_decay'], int(c['decoupled']), int(c['maximize']), None, 0.0,
+                                          state.data_ptr(), 1, lr_t.data_ptr() if on_dev else None, int(t == 4), st)
+
+        if t == 1:
+            _witness_first_launch(call, 'adam_kernel', n, shift)
+        else:
+            N.check(call(), 'adam')
+        Pd, M, V = adam_oracle.adam_step(Pd, G, M, V, t, lr=c['lr'], betas=c['betas'], eps=c['eps'],
+                                         weight_decay=c['weight_decay'], decoupled=c['decoupled'],
+                                         maximize=c['maximize'], coef=1.0)
+    torch.cuda.synchronize()
+    assert int(state[0].item()) == 4 and int(state[1].item()) == 0
+    assert float(g.abs().max().item()) == 0.0  # zero_grad on the last step reached every element
+    err = np.abs(p.cpu().numpy().astype(np.float64) - Pd)
+    bound = 1e-6 * max(np.abs(Pd).max(), 1.0)
+    assert int((err > bound).sum()) <= int(2e-5 * n) and err.max() <= c['lr'], err.max()
+    assert _rel(m.cpu().numpy(), M, 0.1) <= 1e-6 and _rel(v.cpu().numpy(), V, 0.01) <= 1e-6
+    if shift:
+        assert all(float(t[0]) == 0.0 for t in dev)
+
+
+@pytest.mark.parametrize('shift', [0, 1], ids=['vector', 'shifted_scalar'])
+@pytest.mark.parametrize('regime', ['first_multi_sweep', 'resnet18_params'])
+@pytest.mark.parametrize('cfg', [1, 3], ids=['nesterov_wd', 'dampened'])
+def test_sgd_kernel_past_one_sweep(regime, shift, cfg):
+    from dmlcloud_b200 import _native as N
+
+    c = SGD_CONFIGS[cfg]
+    n = _sweep_size(regime)
+    lib, st = N.cuda_lib(0), N.stream_ptr()
+    rng = np.random.RandomState(n % 1000 + 10 * cfg + shift)
+    P = rng.randn(n).astype(np.float32)
+    Pd, Bd = P.astype(np.float64), np.zeros(n)
+    dev = [torch.zeros(n + shift, dtype=torch.float32, device='cuda') for _ in range(3)]
+    p, g, b = (t[shift:] for t in dev)
+    p.copy_(torch.from_numpy(P))
+    b.fill_(123.0)
+    state = torch.zeros(2, dtype=torch.int64, device='cuda')
+    lr_t = torch.full((1,), c['lr'], dtype=torch.float64, device='cuda')
+    for t in range(1, 5):
+        G = (rng.randn(n) * (0.05 if t % 2 else 3.0)).astype(np.float32)
+        g.copy_(torch.from_numpy(G))
+
+        def call():
+            return lib.dmlb_sgd_step_f32(p.data_ptr(), g.data_ptr(), b.data_ptr(), n, 123.0 if t >= 3 else c['lr'],
+                                         c['momentum'], c['dampening'], c['weight_decay'], int(c['nesterov']),
+                                         int(c['maximize']), None, 0.0, state.data_ptr(), 1,
+                                         lr_t.data_ptr() if t >= 3 else None, int(t == 4), st)
+
+        if t == 1:
+            _witness_first_launch(call, 'sgd_kernel', n, shift)
+        else:
+            N.check(call(), 'sgd')
+        Pd, Bd = adam_oracle.sgd_step(Pd, G, Bd, t == 1, coef=1.0, **c)
+    torch.cuda.synchronize()
+    assert int(state[0].item()) == 4
+    assert float(g.abs().max().item()) == 0.0
+    assert _rel(p.cpu().numpy(), Pd, 1.0) <= 2e-6
+    assert _rel(b.cpu().numpy(), Bd, 1.0) <= 2e-6
+    if shift:
+        assert all(float(t[0]) == 0.0 for t in dev)

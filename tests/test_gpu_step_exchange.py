@@ -194,3 +194,137 @@ def test_dead_peer_poisons_the_step_instead_of_hanging():
     res = json.loads((out / 'r0.json').read_text())
     assert res['nan'] and res['failed'] and res['sumsq_nan'], res
     assert res['status'] in (N.METRIC_TIMEOUT, None), res
+
+
+# ----------------------------------------------------------------------------------------------------------------------
+# The metric CTA at its capacity: exactly DMLB_STEP_METRIC_MAX_CELLS global cells fill one 16 KB half of the metric
+# staging area; one more cell must be refused.  Through the LL kernel, the barrier one-shot, the two-shot and a step with
+# no gradients (n = 0).
+# ----------------------------------------------------------------------------------------------------------------------
+def _max_cells_steps(rank, world, dev, wire, n_grad, algo):
+    import torch.distributed as dist
+
+    import launch_geometry as G
+    from dmlcloud_b200 import _native as N
+    from dmlcloud_b200.gradsync import WIRES, PeerComm
+    from dmlcloud_b200.metrics import DeviceSlab, StepRing, _layout_hash
+    from helpers import dmlb_launches
+    from oracle import grad_oracle
+    from oracle.slab_oracle import MAX, MEAN, MIN, SUM, OracleSlab
+
+    lib, st = N.cuda_lib(dev.index), N.stream_ptr()
+    comm = PeerComm(dev, None, max_message_bytes=4 << 20)
+    slab = DeviceSlab(dev)
+    ora = OracleSlab(capacity=4096)
+    blocks = []  # (cell, lanes, k, op): four 255-lane scalar blocks + one 3-lane warp-path fold (k = 33) = 1,023 cells
+    for op in (MEAN, SUM, MIN, MAX):
+        blocks.append((slab.alloc(255, _desc(op, False, True)), 255, 1, op))
+    blocks.append((slab.alloc(3, _desc(MAX, False, True)), 3, 33, MAX))
+    extra = slab.alloc(1, _desc(SUM, False, True))  # the 1,024th global cell (only in the refused descriptor)
+    local = slab.alloc(1, _desc(SUM, True, False))
+    for cell, lanes, k, op in blocks:
+        assert ora.alloc(lanes, _desc(op, False, True)) == cell
+    ora.alloc(1, _desc(SUM, False, True))
+    assert ora.alloc(1, _desc(SUM, True, False)) == local
+    slab.flush()
+    torch.cuda.synchronize()
+    n_glob = sum(b[1] for b in blocks)
+    assert n_glob == G.STEP_METRIC_MAX_CELLS
+    glob, loc = [(0, n_glob)], [(local, local + 1)]
+    h = _layout_hash(('max-cells', n_glob))
+    ring = StepRing(lib, slab.capacity)
+    counter = torch.zeros(1, dtype=torch.int64, device=dev)
+    sumsq = torch.zeros(1, dtype=torch.float64, device=dev)
+    rng = np.random.RandomState(300 + rank)
+    sms = N.device_info(dev.index)['sm_count']
+    ok = {'grad_bit_exact': True, 'metrics_bit_exact': True, 'status_ok': True, 'refused': True}
+    witnessed = []
+
+    def descriptor(ranges, n_global, values):
+        m = N.StepMetrics()
+        m.acc, m.cnt, m.desc = slab.acc.data_ptr(), slab.cnt.data_ptr(), slab.desc.data_ptr()
+        m.counter, m.out_ring, m.feed = counter.data_ptr(), ring.device_ptr, None
+        m.layout_hash, m.n_cells, m.capacity = h, slab.n_cells, slab.capacity
+        m.ring_slots, m.feed_slots = StepRing.SLOTS, 0
+        folds = [N.FoldEntry(v.data_ptr(), 0, N.F32, cell, lanes, k, 1, 0) for (cell, lanes, k, _), v in zip(blocks, values)]
+        folds.append(N.FoldEntry(None, rank + 1, N.F64, local, 1, 1, 1, 0))
+        m.n_folds = len(folds)
+        for i, e in enumerate(folds):
+            m.folds[i] = e
+        m.n_ranges, m.n_global_ranges = len(ranges), n_global
+        for i, (b, e) in enumerate(ranges):
+            m.ranges[i] = N.Range(b, e)
+        return m
+
+    for t in range(1, 3):
+        values = [torch.from_numpy(rng.randn(lanes, k).astype(np.float32)).to(dev) for _, lanes, k, _ in blocks]
+        # 1,024 global cells: refused before any launch, nothing folded
+        before = N.launch_count()
+        too_many = descriptor([(0, n_glob + 1)] + loc, 1, values)
+        assert extra == n_glob
+        rc = lib.dmlb_comm_allreduce(comm.handle, None, 0, WIRES[wire], 1.0, None, algo, ctypes.byref(too_many), st)
+        ok['refused'] &= rc == N.ECAPACITY and N.launch_count() == before
+        g_local = (rng.randn(max(n_grad, 1)) * 3).astype(np.float32)[:n_grad]
+        bucket = torch.from_numpy(g_local.copy()).to(dev) if n_grad else None
+        m = descriptor(glob + loc, 1, values)
+        sumsq.zero_()
+
+        def call():
+            return lib.dmlb_comm_allreduce(comm.handle, bucket.data_ptr() if n_grad else None, n_grad, WIRES[wire],
+                                           1.0 / world, sumsq.data_ptr(), algo, ctypes.byref(m), st)
+
+        rc, launches = dmlb_launches(call)
+        N.check(rc, 'step exchange')
+        proto, grid, _ = G.allreduce_plan(n_grad, wire == 'bf16', world, sms, algo=algo, metrics=True)
+        witnessed.append({'proto': proto, 'grid': grid, 'traced': launches.traced, 'launches': list(launches)})
+        for (cell, lanes, k, _), v in zip(blocks, values):
+            for c in range(lanes):
+                ora._fold(cell + c, v[c].cpu().numpy())
+        ora.acc_i[local] += rank + 1
+        ora.cnt[local] += 1
+        o_status, o_vals, o_flags = ora.reduce(glob, loc, h, reset=False).get()
+        torch.cuda.synchronize()
+        if n_grad:
+            everyone = [None] * world
+            dist.all_gather_object(everyone, g_local) if world > 1 else everyone.__setitem__(0, g_local)
+            stacked = np.stack(everyone)
+            want = grad_oracle.allreduce_f32(stacked) if wire == 'fp32' else \
+                grad_oracle.allreduce_bf16(stacked, round_result=proto == 'twoshot')
+            ok['grad_bit_exact'] &= bool((bucket.cpu().numpy() == want).all())
+        status, vals, flags = ring.read(t)
+        ok['status_ok'] &= status == N.METRIC_OK == o_status
+        sel = [c for b, e in glob + loc for c in range(b, e)]
+        ok['metrics_bit_exact'] &= all(int(vals[c]) == int(o_vals[c]) and int(flags[c]) == int(o_flags[c]) for c in sel)
+    comm.close()
+    return ok, witnessed
+
+
+def _max_cells_worker(rank, world, initfile, outdir, wire, n_grad, algo):
+    init_gloo(rank, world, initfile)
+    import torch.distributed as dist
+
+    torch.cuda.set_device(rank_device(rank))
+    dev = torch.device('cuda', rank_device(rank))
+    ok, witnessed = _max_cells_steps(rank, world, dev, wire, n_grad, algo)
+    Path(outdir, f'r{rank}.json').write_text(json.dumps({'ok': ok, 'witnessed': witnessed}))
+    dist.barrier()
+    dist.destroy_process_group()
+
+
+@pytest.mark.parametrize('world,wire,n_grad,algo', [(2, 'bf16', N_GRAD, 0), (2, 'fp32', N_GRAD, 5), (4, 'fp32', 600_001, 0),
+                                                    (2, 'fp32', 0, 0)],
+                         ids=['ll', 'barrier_oneshot', 'twoshot', 'metrics_only'])
+def test_step_exchange_at_metric_cell_capacity(world, wire, n_grad, algo):
+    from helpers import Launches, check_launches
+
+    out = spawn(_max_cells_worker, world, wire, n_grad, algo, timeout=600)
+    for r in range(world):
+        res = json.loads((out / f'r{r}.json').read_text())
+        assert all(res['ok'].values()), (r, res['ok'])
+        for w in res['witnessed']:
+            launches = Launches([tuple(x) for x in w['launches']])
+            launches.traced = w['traced']
+            (kernel, _), = launches
+            if w['traced']:
+                assert kernel.startswith(f'dmlb::allreduce_{w["proto"]}_kernel<'), (kernel, w)
+            check_launches(launches, [(kernel, w['grid'])])
