@@ -1,4 +1,4 @@
-"""Whole-step CUDA graph for TrainValStage (SURVEY §8f-4) with the fused step exchange.
+"""Whole-step CUDA graphs for TrainValStage (SURVEY §8f-4) with the fused step exchange.
 
 The MNIST-CNN step is ~60 kernel launches of a few microseconds each: eager, it is bounded by Python / launch latency,
 not by the GPU (SURVEY §3.3 "hot spots").  `GraphedTrainStep` captures one training step
@@ -17,18 +17,35 @@ into ONE cudaGraph and replays it per batch.  What is different from the eager l
     barrier of its own: one extra CTA of the all-reduce kernel folds the values, exchanges 16-byte records under the
     gradients' flag barrier and writes the results into a ring in mapped host memory (`stage.live_metrics`);
   * host scalars tracked between replays (misc/step_time_ms, stage.py:314) travel INTO the graph through a second ring
-    in mapped host memory (metrics.HostFeed), one slot per replay — no launch, no copy;
+    in mapped host memory (metrics.HostFeed), one slot per exchange — no launch, no copy;
   * learning rates live in device memory (optim.FlatAdam / FlatSGD), so `scheduler.step()` (stage.py:316-318) takes
     effect on the next replay; a torch optimizer with a python-float lr would have it baked in, which is refused.
 
-Requirements: static batch shapes; FlatAdam / FlatSGD, or torch optimizers constructed with `capturable=True` and no
-scheduler; `step()` must not synchronise with the host (no .item(), no printing of tensors).
+Batches of several shapes — the short last batch of a loader without drop_last, dict batches, batches that carry python
+values — get one graph per batch signature (`batch_signature`: tree structure, (shape, dtype) of every tensor leaf, the
+value of every other leaf).  The first graph is captured on batch `cuda_graph_warmup + 1`.  After that, a signature seen
+for the first time runs `_one_step` UNCAPTURED (the "flat step": same code, same flat bucket, same fused exchange kernel;
+it also lets cuDNN / cuBLAS pick their algorithms for the new shape), is captured on its second occurrence and replayed
+from then on.  Signatures beyond `TrainValStage.cuda_graph_max_shapes`, and batches with an unhashable non-tensor leaf,
+always take the flat step.
+
+Why the ranks stay paired whatever each one decides: every kind of training step — a replay of any signature's graph, a
+flat step, the real run that follows a capture — issues exactly ONE dmlb_comm_allreduce on the flat gradient bucket, with
+the same n (the bucket's size depends on the parameters, not on the batch), the same wire and the same metric descriptor
+layout.  The communicator's sequence number and the exchange counter live in device memory and are shared by all of these
+paths.  So rank 0 may replay the graph of its 8-sample last batch while rank 1 runs its 5-sample last batch as a flat
+step: both issue the same collective.  A step kind that issued a second collective, or none, would break this.
+
+Requirements: FlatAdam / FlatSGD, or torch optimizers constructed with `capturable=True` and no scheduler; `step()` must
+not synchronise with the host (no .item(), no printing of tensors) and must depend on the batch only through its
+signature (shapes, dtypes, python values), as any captured code must.
 """
 import ctypes
 
 import torch
 import torch.distributed as dist
 from torch.nn.parallel import DistributedDataParallel
+from torch.utils._pytree import tree_flatten, tree_unflatten
 
 from . import _native as N
 from .gradsync import WIRES, PeerComm
@@ -57,8 +74,48 @@ class FlatGradBucket:
         return all(p.grad is not None and p.grad.untyped_storage().data_ptr() == base for p in self.params)
 
 
+def batch_signature(batch):
+    """(key, leaves) of a training batch.  `key` names the graph the batch can replay: the batch's pytree structure, then
+    per leaf (shape, dtype) for a tensor and the value itself for anything else.  It is None when a non-tensor leaf is
+    unhashable: such a batch never gets a graph.  `leaves` is the batch's flat list of leaves (torch.utils._pytree order).
+
+    A flat tuple or list of tensors — what a DataLoader yields — is keyed by its type instead of its tree spec, which says
+    nothing more there; that takes about a microsecond per step instead of the six of a full tree_flatten."""
+    if type(batch) is tuple or type(batch) is list:
+        key = [(x.shape, x.dtype) if isinstance(x, torch.Tensor) else None for x in batch]
+        if None not in key:
+            return (type(batch), tuple(key)), batch
+    leaves, spec = tree_flatten(batch)
+    key = []
+    for x in leaves:
+        if isinstance(x, torch.Tensor):
+            key.append((tuple(x.shape), x.dtype))
+            continue
+        try:
+            hash(x)
+        except TypeError:
+            return None, leaves
+        key.append(x)
+    return (spec, tuple(key)), leaves
+
+
+class _ShapeGraph:
+    """What belongs to ONE batch signature: its static inputs, its graph and what the graph's nodes point at."""
+
+    def __init__(self):
+        self.leaves = None        # static inputs: device tensors (non-tensor leaves as the loader gave them)
+        self.batch = None         # the same leaves in the loader's structure: what train_step receives
+        self.graph = None
+        self.loss = None
+        self.step_metrics = None  # the dmlb_step_metrics descriptor baked into the graph (None: no live exchange)
+        self.live_names = {}
+        self.keep = None          # tensors the captured fold entries read: they must live as long as the graph
+        self.kernels = 0          # libdmlb kernels one replay re-runs
+        self.replays = 0
+
+
 class GraphedTrainStep:
-    def __init__(self, stage, example_batch):
+    def __init__(self, stage):
         self.stage = stage
         pipeline = stage.pipeline
         self.device = pipeline.device
@@ -104,40 +161,84 @@ class GraphedTrainStep:
                                'gradient set that fits grad_arena_bytes')
         self.comm = comm
         self.sumsq = torch.zeros(1, dtype=torch.float64, device=self.device)
-        self.static = tuple(torch.empty_like(t, device=self.device) if isinstance(t, torch.Tensor) else t
-                            for t in example_batch)
-        self.graph = None
-        self.loss = None
-        self.replays = 0
+        self.shapes = {}   # batch signature -> _ShapeGraph (graph None: seen once, or dropped when the slab grew)
+        self.first = None  # the first captured signature: `graph`, `step_metrics` and `kernels_in_graph` describe it
+        self.loss = None   # the loss of the latest step, whichever kind it was
+        self.replays = 0   # graph-driven steps of every signature, the real run after each capture included
+        self.flat_steps = 0
+        self.captures = 0
+        self.exchanges = 0  # fused step exchanges with a metric descriptor == the device counter's value
         self.kernels_in_graph = 0
-        # fused step exchange state (built at capture)
+        # fused step exchange state, shared by every signature and by the flat step (created once, before the first step)
         self.ring = None
         self.feed = None
         self.counter = None
-        self.replays_at_ring = 0
+        self._landed = 0  # exchanges known to have completed when the current ring was created
         self.live_names = {}
         self.zero_in_optimizer = False
+        self._feed_fixed = False  # the feed's column map is assigned: every graph and flat step uses that same map
+        self._pool = None
         self._copy_stream = None  # side stream + double-buffered staging for large pinned host batches (see _load)
         self._staging = {}
         self._slab_generation = None
-        self._keep = None
-        self.step_metrics = None
+        self._said = set()
+
+    @property
+    def graph(self):
+        return self.first.graph if self.first is not None else None
+
+    @property
+    def step_metrics(self):
+        return self.first.step_metrics if self.first is not None else None
+
+    @property
+    def static(self):
+        return self.first.batch if self.first is not None else None
 
     def _wire_bytes(self, n):
         return ((n + 7) // 8) * 16 if self.wire == 'bf16' else ((n + 3) // 4) * 16
 
+    def _say(self, what, message):
+        if what not in self._said:
+            self._said.add(what)
+            self.stage.logger.warning(message)
+
     # ---- the fused step exchange -------------------------------------------------------------------------------------
+    def _prepare_exchange(self, slab):
+        """Exchange counter, host feed and result ring: created once, outside any capture (pinned memory cannot be
+        allocated while a stream captures, and a tensor made inside a capture would be re-initialised by every replay).
+        Every graph bakes in their addresses, so they are never replaced — except the ring, when the slab grew and every
+        graph is captured again anyway."""
+        if self.counter is None:
+            self.counter = torch.zeros(1, dtype=torch.int64, device=self.device)
+        if self.stage.live_metrics_every:
+            if self.feed is None:
+                self.feed = HostFeed(self.lib)
+            if self.ring is None or self.ring.capacity != slab.capacity:
+                self._new_ring(slab.capacity)
+
+    def _new_ring(self, capacity):
+        if self.ring is not None:
+            if torch.cuda.is_current_stream_capturing():
+                raise RuntimeError('cuda_graph mode: the metric slab grew while a step was being captured')
+            torch.cuda.synchronize(self.device)  # exchanges still in flight write into the old ring
+            self._landed = self.exchanges
+        self.ring = StepRing(self.lib, capacity)
+
     def _describe_metrics(self, entries):
-        """dmlb_step_metrics for this step: the queued fold entries + the live selection + the two host rings."""
+        """(dmlb_step_metrics for this step, {name: metric} it covers): the queued fold entries + the live selection + the
+        two host rings.  (None, {}) when the step has no live exchange."""
         tracker = self.stage.tracker
         slab = tracker._slab_or_create()
         by_name, plan = tracker.live_selection()
         if not by_name:
-            return None
+            return None, {}
         glob, loc, layout = plan
         n_glob = sum(e - b for b, e in glob)
         if n_glob > N.STEP_METRIC_MAX_CELLS or len(glob) + len(loc) > N.MAX_RANGES or len(entries) > N.MAX_FOLD_ENTRIES:
-            return None  # too large for the piggy-back: the stage falls back to the separate exchange kernel
+            return None, {}  # too large for the piggy-back: the stage falls back to the separate exchange kernel
+        if self.ring.capacity != slab.capacity:
+            self._new_ring(slab.capacity)  # a metric first tracked in this (uncaptured) step grew the slab
         m = N.StepMetrics()
         m.acc, m.cnt, m.desc = slab.acc.data_ptr(), slab.cnt.data_ptr(), slab.desc.data_ptr()
         m.counter = self.counter.data_ptr()
@@ -153,8 +254,24 @@ class GraphedTrainStep:
         m.n_ranges, m.n_global_ranges = len(ranges), len(glob)
         for i, (b, e) in enumerate(ranges):
             m.ranges[i] = N.Range(b, e)
-        self.live_names = dict(by_name)
-        return m
+        return m, dict(by_name)
+
+    def _before_exchange(self):
+        count = self.exchanges  # exchanges issued so far == the counter value this one reads == its feed slot
+        if count % 16 == 0 and count - self.counter_host() >= HostFeed.SLOTS // 2:
+            # the host is half a ring ahead of the GPU: wait for the exchange that frees the slot about to be written
+            self.ring.wait(count - HostFeed.SLOTS // 2 + 1, sync=lambda: torch.cuda.synchronize(self.device))
+        self.feed.commit(count)
+
+    def _after_exchange(self, live_names):
+        self.exchanges += 1
+        self.live_names = live_names
+        self.stage.live_metrics = self.stage.tracker.live_view(
+            _RingResult(self.ring, self.exchanges, sync=lambda: torch.cuda.synchronize(self.device)), live_names)
+
+    def counter_host(self):
+        """Number of step exchanges the GPU has completed, read from the result ring's stamps (no CUDA call)."""
+        return max(self.ring.latest(), self._landed) if self.ring is not None else 0
 
     def _sync_gradients(self, metrics=None):
         flat, n = self.bucket.flat, self.bucket.total
@@ -183,7 +300,9 @@ class GraphedTrainStep:
                     clip = None
                 opt.step()
 
-    def _one_step(self):
+    def _one_step(self, batch, eager):
+        """One training step on `batch` (captured, or run as it is when `eager`): (loss, step metrics descriptor, live
+        names, tensors the fold entries read)."""
         stage = self.stage
         slab = stage.tracker._slab_or_create()
         if not self.zero_in_optimizer:
@@ -196,7 +315,7 @@ class GraphedTrainStep:
             for c in ctxs:
                 c.__enter__()
             try:
-                loss = stage.train_step(self.static)
+                loss = stage.train_step(batch)
                 loss.backward()
             finally:
                 for c in reversed(ctxs):
@@ -207,30 +326,79 @@ class GraphedTrainStep:
         finally:
             slab.batching = False
         if self.feed is not None:
-            # python scalars the stage tracks BETWEEN steps (misc/step_time_ms, stage.py:314) get a column of the host feed
-            # ring; the ones tracked inside the step (the batch counters) are immediates of this very fold
-            inside = {e.cell for e in entries if not e.src}
-            cols = {c: kind for c, kind in slab.imm_cells_seen.items() if c not in inside}
-            room = N.MAX_FOLD_ENTRIES - len(entries)
-            cols = dict(sorted(cols.items())[:max(0, min(N.FEED_WIDTH, room))])
-            self.feed.assign(cols)
+            if not self._feed_fixed:
+                # python scalars the stage tracks BETWEEN steps (misc/step_time_ms, stage.py:314) get a column of the host
+                # feed ring; the ones tracked inside the step (the batch counters) are immediates of this very fold.  The
+                # map is assigned once and shared by every graph and flat step: a graph bakes in "column j is cell X"
+                inside = {e.cell for e in entries if not e.src}
+                cols = {c: kind for c, kind in slab.imm_cells_seen.items() if c not in inside}
+                room = N.MAX_FOLD_ENTRIES - len(entries)
+                cols = dict(sorted(cols.items())[:max(0, min(N.FEED_WIDTH, room))])
+                self.feed.assign(cols)
             for cell, j in self.feed.cols.items():
                 entries.append(N.FoldEntry(None, 0, N.SRC_FEED, cell, 1, j, 1, 0))
-        metrics = self._describe_metrics(entries) if stage.live_metrics_every else None
+        metrics, live_names = self._describe_metrics(entries) if stage.live_metrics_every else (None, {})
         if metrics is None:  # no live exchange wanted (or it does not fit): plain fold launch(es), inside the graph
-            if self.feed is not None:
+            if self.feed is not None and not self._feed_fixed:
                 self.feed.assign({})  # nobody would read the feed ring: python scalars keep their normal route
+            # (with the map already in use, the feed's scalars wait for the next step that has an exchange)
             real = [e for e in entries if e.src_dtype != N.SRC_FEED]
             for i in range(0, len(real), N.MAX_FOLD_ENTRIES):
                 slab._launch_fold(real[i:i + N.MAX_FOLD_ENTRIES])
-        self.step_metrics, self._keep = metrics, keep
+        elif eager:
+            self._before_exchange()
+        if self.feed is not None:
+            self._feed_fixed = True
         self._sync_gradients(metrics)
         self._optimize()
-        return loss
+        return loss, metrics, live_names, keep
+
+    # ---- the three kinds of step -------------------------------------------------------------------------------------
+    def __call__(self, batch):
+        key, leaves = batch_signature(batch)
+        slab = self.stage.tracker._slab_or_create()
+        if slab.generation != self._slab_generation:
+            self._invalidate(slab)
+        self._sync_lr()
+        shape = self.shapes.get(key) if key is not None else None
+        if shape is not None and shape.graph is not None:
+            self._load(key, shape, leaves)
+            self._replay(shape)
+        elif shape is not None or (key is not None and self.first is None):
+            self._capture(key, batch, leaves)  # second occurrence, first graph of all, or again after the slab grew
+        else:
+            if key is None:
+                self._say('unhashable', 'cuda_graph mode: a batch with an unhashable non-tensor leaf runs uncaptured')
+            elif len(self.shapes) < self.stage.cuda_graph_max_shapes:
+                self.shapes[key] = _ShapeGraph()  # captured on its next occurrence
+            else:
+                self._say('cap', f'cuda_graph mode: more than cuda_graph_max_shapes = {self.stage.cuda_graph_max_shapes} '
+                                 'batch shapes; further shapes run uncaptured')
+            self._flat_step(batch)
+        return self.loss
 
     def capture(self, batch):
-        """Capture the step on `batch` (its values are consumed: this is a real training step)."""
-        self._load(batch)
+        """Capture the step for `batch`'s signature on `batch` (its values are consumed: this is a real training step)."""
+        key, leaves = batch_signature(batch)
+        if key is None:
+            raise RuntimeError('cuda_graph mode: a batch with an unhashable non-tensor leaf cannot be captured')
+        self._sync_lr()
+        return self._capture(key, batch, leaves)
+
+    def _sync_lr(self):
+        for opt in self.stage.optimizers():
+            sync_lr = getattr(opt, 'sync_device_lr', None)
+            if sync_lr is not None:
+                sync_lr()  # a scheduler changed group['lr']: one tiny fill, only when the value actually changed
+
+    def _capture(self, key, batch, leaves):
+        shape = self.shapes.get(key)
+        if shape is None:
+            shape = self.shapes[key] = _ShapeGraph()
+        if shape.leaves is None:
+            shape.leaves = [torch.empty_like(x, device=self.device) if isinstance(x, torch.Tensor) else x for x in leaves]
+            shape.batch = tree_unflatten(shape.leaves, tree_flatten(batch)[1])
+        self._load(key, shape, leaves)
         if not self.bucket.attached():
             raise RuntimeError('cuda_graph mode: parameter .grad no longer alias the flat bucket')
         stream = torch.cuda.current_stream(self.device)
@@ -241,62 +409,96 @@ class GraphedTrainStep:
         slab = stage.tracker._slab_or_create()
         # host scalars queued by the last eager step must be launched NOW: inside the capture they would be baked into
         # the graph and re-added by every replay
-        slab.flush_all()  # (also hands scalars still waiting in a previous capture's feed ring to a normal fold launch)
+        slab.flush_all()  # (also hands scalars still waiting in the feed ring to a normal fold launch)
         slab.feed = None
-        for opt in stage.optimizers():
-            sync_lr = getattr(opt, 'sync_device_lr', None)
-            if sync_lr is not None:
-                sync_lr()
-        # pinned memory cannot be allocated while a stream is capturing: the host feed ring exists before the capture, its
-        # columns are assigned inside it (when the step has shown which python scalars it tracks itself)
-        self.feed = HostFeed(self.lib) if stage.live_metrics_every else None
-        # result ring (mapped host memory) and exchange counter (device) of the fused step exchange: created OUTSIDE the
-        # capture — a tensor made inside it would be re-initialised by every replay
-        self.ring = StepRing(self.lib, slab.capacity) if stage.live_metrics_every else None
-        self.counter = torch.zeros(1, dtype=torch.int64, device=self.device)
-        self.replays_at_ring = self.replays
+        self._prepare_exchange(slab)
+        if self.first is None:
+            # DDP rebuilds its buckets in the first forward after the first backward, with a host-to-device copy that
+            # cannot be captured: with cuda_graph_warmup = 1 that forward is the capture's, so do it here (all ranks
+            # capture their first graph at the same step; afterwards the call returns at once)
+            for m in self.ddp_models:
+                m.reducer._rebuild_buckets()
         torch.cuda.synchronize(self.device)
-        # `optimizer.zero_grad()` of the next step (reference stage.py:300) is fused into the K5 / K6 launch when ONE flat
-        # optimizer owns every gradient of the bucket: one kernel node and one pass over the gradients fewer per step
-        opts = list(stage.optimizers())
-        self.zero_in_optimizer = (len(opts) == 1 and getattr(opts[0], 'device_lr', False) and len(opts[0].param_groups) == 1
-                                  and opts[0]._flat_grad_base(opts[0].param_groups[0], opts[0]._flat[0]) ==
-                                  self.bucket.flat.data_ptr() and opts[0]._flat[0]['total'] == self.bucket.total)
-        if self.zero_in_optimizer:
-            opts[0].zero_grad_in_step = True
-            self.bucket.flat.zero_()  # once, outside the graph: every replay leaves zeros behind
-        self.graph = torch.cuda.CUDAGraph()
+        if self.first is None:
+            # `optimizer.zero_grad()` of the next step (reference stage.py:300) is fused into the K5 / K6 launch when ONE
+            # flat optimizer owns every gradient of the bucket: one kernel node and one pass over the gradients fewer
+            opts = list(stage.optimizers())
+            self.zero_in_optimizer = (len(opts) == 1 and getattr(opts[0], 'device_lr', False)
+                                      and len(opts[0].param_groups) == 1
+                                      and opts[0]._flat_grad_base(opts[0].param_groups[0], opts[0]._flat[0]) ==
+                                      self.bucket.flat.data_ptr() and opts[0]._flat[0]['total'] == self.bucket.total)
+            if self.zero_in_optimizer:
+                opts[0].zero_grad_in_step = True
+                self.bucket.flat.zero_()  # once, outside the graph: every replay and flat step leaves zeros behind
+        # All graphs share one memory pool.  A capture may reuse memory another capture freed (its intermediates), never
+        # memory another graph still holds (its loss, the tensors its fold entries read).  That is safe because the graphs
+        # replay one at a time on one stream and no graph's intermediates are read after another graph has replayed;
+        # the loss of a step is its own graph's output, which no other graph writes.
+        if self._pool is None:
+            self._pool = torch.cuda.graph_pool_handle()
+        graph = torch.cuda.CUDAGraph()
         # capture on the very stream the warm-up steps ran on: autograd's AccumulateGrad nodes (stashed by DDP at
         # construction) then already live on the capturing stream and no cross-stream edge enters the graph
         before = N.launch_count()
-        with torch.cuda.graph(self.graph, stream=stream):
-            self.loss = self._one_step()
-        self.kernels_in_graph = N.launch_count() - before  # libdmlb kernels every replay re-runs
+        with torch.cuda.graph(graph, pool=self._pool, stream=stream):
+            loss, metrics, live_names, keep = self._one_step(shape.batch, eager=False)
+        shape.kernels = N.launch_count() - before  # libdmlb kernels every replay re-runs
+        shape.graph, shape.loss, shape.step_metrics, shape.live_names, shape.keep = graph, loss, metrics, live_names, keep
+        self.captures += 1
+        if self.first is None:
+            self.first = shape
+        if shape is self.first:
+            self.kernels_in_graph = shape.kernels
+        elif shape.kernels != self.first.kernels:
+            self._say(('kernels', key), f'cuda_graph mode: the graph of batch signature {key} re-runs {shape.kernels} '
+                                        f'libdmlb kernels per replay, the first graph {self.first.kernels}')
         self._slab_generation = slab.generation
-        slab.feed = self.feed  # from now on python scalars of the feed's cells wait for the next replay
-        self._replay()  # capture only records: run the step once for real
+        slab.feed = self.feed  # from now on python scalars of the feed's cells wait for the next exchange
+        self._replay(shape)  # capture only records: run the step once for real
         return self.loss
 
-    def _replay(self):
-        if self.feed is not None and self.step_metrics is not None:
-            count = self.replays_since_ring()  # exchanges issued so far == the slot index the device will use
-            if count % 16 == 0 and count - self.counter_host() >= HostFeed.SLOTS // 2:
-                # the host is half a ring ahead of the GPU: wait for the exchange that frees the slot about to be written
-                self.ring.wait(count - HostFeed.SLOTS // 2 + 1, sync=lambda: torch.cuda.synchronize(self.device))
-            self.feed.commit(count)
-        self.graph.replay()
+    def _replay(self, shape):
+        exchange = shape.step_metrics is not None
+        if exchange:
+            self._before_exchange()
+        shape.graph.replay()
         self.replays += 1
-        if self.step_metrics is not None:
-            k = self.replays_since_ring()
-            self.stage.live_metrics = self.stage.tracker.live_view(
-                _RingResult(self.ring, k, sync=lambda: torch.cuda.synchronize(self.device)), self.live_names)
+        shape.replays += 1
+        self.loss = shape.loss
+        if exchange:
+            self._after_exchange(shape.live_names)
 
-    def replays_since_ring(self):
-        return self.replays - self.replays_at_ring
+    def _flat_step(self, batch):
+        """The step of a signature without a graph, run as it is: the same `_one_step` on the same flat bucket and the
+        same single fused exchange as a replay, so the ranks' collectives stay paired."""
+        leaves, spec = tree_flatten(batch)
+        batch = tree_unflatten([x.to(self.device, non_blocking=True) if isinstance(x, torch.Tensor) else x
+                                for x in leaves], spec)
+        slab = self.stage.tracker._slab_or_create()
+        self._prepare_exchange(slab)
+        assign = self.feed is not None and not self._feed_fixed
+        if assign:  # the feed's column map is assigned by this step: scalars tracked so far take the normal route
+            slab.flush_all()
+            slab.feed = None
+        loss, metrics, live_names, _ = self._one_step(batch, eager=True)  # (the allocator is stream-ordered: the fold
+        if assign:                                                        # entries' tensors may go once it is launched)
+            slab.feed = self.feed
+        self.flat_steps += 1
+        self.loss = loss
+        if metrics is not None:
+            self._after_exchange(live_names)
 
-    def counter_host(self):
-        """Number of step exchanges the GPU has completed, read from the result ring's stamps (no CUDA call)."""
-        return self.ring.latest() if self.ring is not None else 0
+    def _invalidate(self, slab):
+        """The metric slab was reallocated (it grew): every graph holds stale pointers.  Drop them all; each signature is
+        captured again on its next occurrence, without a second warm-up."""
+        if any(s.graph is not None for s in self.shapes.values()):
+            torch.cuda.synchronize(self.device)
+            for s in self.shapes.values():
+                s.graph = s.loss = s.step_metrics = s.keep = None
+                s.live_names = {}
+            self._pool = None
+            self._feed_fixed = False  # no graph holds the column map any more: the next step assigns it afresh
+        self._slab_generation = slab.generation
 
     def time_gradient_sync(self, reps=20, per_graph=20):
         """Device time (us) of ONE gradient-sync launch on the flat bucket (without the metric CTA): `per_graph` of them
@@ -325,14 +527,16 @@ class GraphedTrainStep:
 
     STAGE_MIN_BYTES = 1 << 20
 
-    def _load(self, batch):
-        """Bring `batch` into the captured step's static input buffers.  Large batches that sit in PINNED host memory
-        (ResNet-18: 38.5 MB per step) take a detour that hides the PCIe transfer: the H2D copy goes to one of two staging
-        buffers on a copy stream — the host issues it while the GPU is still computing the previous step — and the
-        compute stream only does a device-to-device copy (microseconds) once the staged data has landed."""
-        for i, (dst, src) in enumerate(zip(self.static, batch)):
+    def _load(self, key, shape, leaves):
+        """Bring the batch's leaves into the static input buffers of its own signature's graph.  Large batches that sit
+        in PINNED host memory (ResNet-18: 38.5 MB per step) take a detour that hides the PCIe transfer: the H2D copy goes
+        to one of two staging buffers on a copy stream — the host issues it while the GPU is still computing the previous
+        step — and the compute stream only does a device-to-device copy (microseconds) once the staged data has landed."""
+        for i, (dst, src) in enumerate(zip(shape.leaves, leaves)):
             if not isinstance(dst, torch.Tensor):
                 continue
+            # the signature matched, so the shapes do: copy_ would otherwise broadcast a smaller batch silently
+            assert dst.shape == src.shape and dst.dtype == src.dtype, (key, i, dst.shape, src.shape)
             staged = (isinstance(src, torch.Tensor) and not src.is_cuda and src.is_pinned()
                       and src.numel() * src.element_size() >= self.STAGE_MIN_BYTES)
             if not staged:
@@ -340,11 +544,12 @@ class GraphedTrainStep:
                 continue
             if self._copy_stream is None:
                 self._copy_stream = torch.cuda.Stream(device=self.device)
-            slot = self._staging.get(i)
+            slot = self._staging.get((key, i))
             if slot is None:
-                slot = self._staging[i] = {'buf': [torch.empty_like(dst), torch.empty_like(dst)], 'next': 0,
-                                           'ready': [torch.cuda.Event(), torch.cuda.Event()],
-                                           'consumed': [torch.cuda.Event(), torch.cuda.Event()], 'used': [False, False]}
+                slot = self._staging[key, i] = {'buf': [torch.empty_like(dst), torch.empty_like(dst)], 'next': 0,
+                                                'ready': [torch.cuda.Event(), torch.cuda.Event()],
+                                                'consumed': [torch.cuda.Event(), torch.cuda.Event()],
+                                                'used': [False, False]}
             k = slot['next']
             slot['next'] ^= 1
             compute = torch.cuda.current_stream(self.device)
@@ -358,28 +563,22 @@ class GraphedTrainStep:
             slot['consumed'][k].record(compute)
             slot['used'][k] = True
 
-    def __call__(self, batch):
-        slab = self.stage.tracker._slab_or_create()
-        if slab.generation != self._slab_generation:
-            # the metric slab was reallocated (it grew): the graph holds stale pointers -> capture again on this batch
-            return self.capture(batch)
-        for opt in self.stage.optimizers():
-            sync_lr = getattr(opt, 'sync_device_lr', None)
-            if sync_lr is not None:
-                sync_lr()  # a scheduler changed group['lr']: one tiny fill, only when the value actually changed
-        self._load(batch)
-        self._replay()
-        return self.loss
-
     def detach(self):
-        """End of the stage: scalars still waiting for a replay take the normal route; later stages see a plain slab."""
+        """End of the stage: scalars still waiting for an exchange take the normal route; later stages see a plain slab.
+        The graphs stay: the stage may train again."""
         slab = self.stage.tracker._slab
         if slab is not None and slab.feed is not None and slab.feed is self.feed:
             slab.flush_all()
             slab.feed = None
 
     def close(self):
+        """detach() and release every signature's graph, static inputs and staging buffers."""
         self.detach()
+        torch.cuda.synchronize(self.device)
+        self.shapes.clear()
+        self._staging.clear()
+        self.first = None
+        self._pool = None
         if self._own_comm is not None:
             self._own_comm.close()
             self._own_comm = None

@@ -178,7 +178,9 @@ class TrainValStage(Stage):
         self.live_metrics = {}
         self.global_step = 0
         # Extension (SURVEY §8f-4): capture the whole training step into one CUDA graph after `cuda_graph_warmup` eager
-        # steps and replay it per batch (graphstep.GraphedTrainStep).  Needs static batch shapes, capturable optimizers.
+        # steps and replay it per batch (graphstep.GraphedTrainStep).  Needs capturable optimizers.  Batches of another
+        # shape (a short last batch) run uncaptured once, then get a graph of their own, up to `cuda_graph_max_shapes`
+        # graphs; further shapes always run uncaptured.
         # Extension: keep Python's cyclic garbage collector out of the step loop.  A generation-2 collection is tens of
         # milliseconds; in a data-parallel run every rank waits for it at the next gradient barrier, and with W ranks it
         # happens W times as often.  True: the collector is disabled while `train_epoch` runs and run once per epoch
@@ -186,6 +188,7 @@ class TrainValStage(Stage):
         self.manual_gc = False
         self.cuda_graph = False
         self.cuda_graph_warmup = 3
+        self.cuda_graph_max_shapes = 4
         self._graph = None
         self._eager_steps = 0
 
@@ -277,10 +280,8 @@ class TrainValStage(Stage):
                 return False
             from .graphstep import GraphedTrainStep
 
-            self._graph = GraphedTrainStep(self, batch)
-            self._graph.capture(batch)
-            return True
-        self._graph(batch)
+            self._graph = GraphedTrainStep(self)
+        self._graph(batch)  # replay, capture or uncaptured step, by the batch's signature
         return True
 
     # ---- epochs ------------------------------------------------------------------------------------------------------
