@@ -1,5 +1,6 @@
 // Device-side pieces of the metric slab shared by metric_kernels.cu (stand-alone fold / reduce launches) and
-// peer_comm.cu (the fused step exchange: a metric CTA rides along with the gradient all-reduce).
+// peer_comm.cu (the fused step exchange: a metric CTA rides along with the gradient all-reduce): the per-cell arithmetic
+// and the cross-rank exchange built on it.
 //
 // Reference arithmetic being replaced (dmlcloud/metrics.py): MetricReducer.append 66-73, reduce_locally 107-119,
 // reduce_globally 121-141 — see metric_kernels.cu for the mapping.
@@ -179,44 +180,40 @@ __device__ __forceinline__ void finalize_cell(uint64_t *acc, long long *cnt, uin
     }
 }
 
-// combine W records of one cell in rank order.  rec(r) -> (val, cnt)
+// One record as it travels: a cell's {val, cnt}, or the header {layout hash, global cell count}.
+struct Record {
+    uint64_t v, n;
+};
+
+// combine W records of one cell in rank order.  rec(r) -> Record of rank r
 template <class Rec>
 __device__ __forceinline__ void combine_cell(uint32_t d, int world, Rec rec, uint64_t &out, uint8_t &flag, int &status) {
     const int op = desc_op(d);
-    int empty = 0;
-    uint64_t v0;
-    long long n0;
-    rec(0, v0, n0);
-    empty += n0 <= 0;
+    const Record x0 = rec(0);
+    int empty = (long long)x0.n <= 0;
     if (desc_int(d)) {
-        long long a = (long long)v0;
+        long long a = (long long)x0.v;
         for (int r = 1; r < world; ++r) {
-            uint64_t v;
-            long long n;
-            rec(r, v, n);
-            empty += n <= 0;
-            a = combine_i(op == DMLB_MEAN ? DMLB_SUM : op, a, (long long)v);
+            const Record x = rec(r);
+            empty += (long long)x.n <= 0;
+            a = combine_i(op == DMLB_MEAN ? DMLB_SUM : op, a, (long long)x.v);
         }
         out = (uint64_t)a;
     } else if (desc_f64(d)) {
-        double a = __longlong_as_double((long long)v0);
+        double a = __longlong_as_double((long long)x0.v);
         for (int r = 1; r < world; ++r) {
-            uint64_t v;
-            long long n;
-            rec(r, v, n);
-            empty += n <= 0;
-            a = combine_f(op == DMLB_MEAN ? DMLB_SUM : op, a, __longlong_as_double((long long)v));
+            const Record x = rec(r);
+            empty += (long long)x.n <= 0;
+            a = combine_f(op == DMLB_MEAN ? DMLB_SUM : op, a, __longlong_as_double((long long)x.v));
         }
         if (op == DMLB_MEAN) a /= (double)world;
         out = (uint64_t)__double_as_longlong(a);
     } else {  // fp32 metric: the cross-rank arithmetic is fp32, like gloo's all_reduce + `tensor /= W`
-        float a = (float)__longlong_as_double((long long)v0);
+        float a = (float)__longlong_as_double((long long)x0.v);
         for (int r = 1; r < world; ++r) {
-            uint64_t v;
-            long long n;
-            rec(r, v, n);
-            empty += n <= 0;
-            float b = (float)__longlong_as_double((long long)v);
+            const Record x = rec(r);
+            empty += (long long)x.n <= 0;
+            float b = (float)__longlong_as_double((long long)x.v);
             if (op == DMLB_MIN)
                 a = (float)nan_min(a, b);
             else if (op == DMLB_MAX)
@@ -229,6 +226,144 @@ __device__ __forceinline__ void combine_cell(uint32_t d, int world, Rec rec, uin
     }
     flag = empty == world ? 1 : 0;
     if (empty != 0 && empty != world) status = DMLB_METRIC_SPLIT_VOTE;
+}
+
+// ---------------------------------------------------------------------------------------------------------------------
+// The metric exchange, one routine for every path that reduces metrics across ranks.  Each rank finalises the selected
+// cells and publishes a header {layout hash, global cell count} plus one 16-byte record {val, cnt} per global cell; each
+// rank then checks every peer's header, combines the records in rank order and collapses its threads' status into one
+// code.  The transport is the sink and loaders its caller passes in:
+//   metric_reduce_kernel (K4)          records in this rank's staging half, per-CTA flag barrier    (metric_kernels.cu)
+//   metric_cta<false> / <true>         records in mstage under the all-reduce's barrier 0 / LL lines (peer_comm.cu)
+//   metric_finalize / combine_kernel   a record buffer the caller all-gathers (torch.distributed)    (metric_kernels.cu)
+// ---------------------------------------------------------------------------------------------------------------------
+
+// A selection: [global ranges | rank-local ranges].  Global cells are exchanged; rank-local ones never are.
+struct Selection {
+    const dmlb_range *r;
+    int n_ranges, n_global_ranges;
+    int n_glob, n_loc;
+    __device__ __forceinline__ int glob_cell(int i) const { return sel_to_cell(r, n_global_ranges, i); }
+    __device__ __forceinline__ int loc_cell(int i) const {
+        return sel_to_cell(r + n_global_ranges, n_ranges - n_global_ranges, i);
+    }
+};
+
+__device__ __forceinline__ Selection count_selection(const dmlb_range *r, int n_ranges, int n_global_ranges) {
+    Selection S{r, n_ranges, n_global_ranges, 0, 0};
+    for (int j = 0; j < n_ranges; ++j) (j < n_global_ranges ? S.n_glob : S.n_loc) += r[j].end - r[j].begin;
+    return S;
+}
+
+// Host side: checks a selection's ranges (each inside [0, limit)), counts its global and rank-local cells and copies the
+// ranges to `copy` (when given).
+inline int check_selection(const dmlb_range *r, int n_ranges, int n_global_ranges, long long limit, long long &n_glob,
+                           long long &n_loc, dmlb_range *copy = nullptr) {
+    if (n_ranges < 0 || n_ranges > DMLB_MAX_RANGES || (n_ranges > 0 && !r) || n_global_ranges < 0 ||
+        n_global_ranges > n_ranges)
+        return DMLB_ECAPACITY;
+    n_glob = n_loc = 0;
+    for (int j = 0; j < n_ranges; ++j) {
+        if (r[j].begin < 0 || r[j].end < r[j].begin || r[j].end > limit) return DMLB_EINVAL;
+        (j < n_global_ranges ? n_glob : n_loc) += r[j].end - r[j].begin;
+        if (copy) copy[j] = r[j];
+    }
+    return DMLB_OK;
+}
+
+// A result block: int32 status[DMLB_METRIC_STATUS_SLOTS] | u64 val[C] | u8 flag[C].  A step-ring slot keeps its stamp in
+// the last 8 status bytes.
+struct Results {
+    int *status;
+    uint64_t *val;
+    uint8_t *flag;
+    static constexpr size_t kStatusBytes = (size_t)DMLB_METRIC_STATUS_SLOTS * 4;
+    __device__ static size_t bytes(int capacity) { return kStatusBytes + 9 * (size_t)capacity; }
+    __device__ static Results block(unsigned char *base, int capacity) {
+        return {reinterpret_cast<int *>(base), reinterpret_cast<uint64_t *>(base + kStatusBytes),
+                base + kStatusBytes + 8 * (size_t)capacity};
+    }
+    __device__ volatile unsigned long long *stamp() const {
+        return reinterpret_cast<volatile unsigned long long *>(status + DMLB_METRIC_STATUS_SLOTS) - 1;
+    }
+    __device__ __forceinline__ void put(int cell, uint64_t v, uint8_t f) const { val[cell] = v, flag[cell] = f; }
+    // Status slots are sticky (max with what is there), so that a reduce split over several launches keeps an error of
+    // an earlier launch; the caller zeroes them per reduce.  A clean run leaves its slot untouched.
+    __device__ __forceinline__ void raise(int slot, int st) const {
+        if (threadIdx.x == 0 && st != DMLB_METRIC_OK && st > status[slot]) status[slot] = st;
+    }
+};
+
+__device__ __forceinline__ uint64_t u64_of(uint32_t lo, uint32_t hi) { return ((uint64_t)hi << 32) | lo; }
+
+// Staged records (a staging half, mstage, or one rank's part of the gathered buffer): u64 words {hash, n_glob}, then
+// {val, cnt} per global selection index.  Each is 16 bytes, so the header is record -1.
+__device__ __forceinline__ void put_record(uint64_t *rec, int i, uint64_t v, uint64_t n) {
+    rec[2 + 2 * i] = v;
+    rec[3 + 2 * i] = n;
+}
+__device__ __forceinline__ Record staged(uint4 w) { return {u64_of(w.x, w.y), u64_of(w.z, w.w)}; }
+__device__ __forceinline__ Record load_staged(const unsigned char *base, int i) {
+    return staged(ld_coherent_u4(reinterpret_cast<const uint4 *>(base) + 1 + i));
+}
+
+// Finalise indices first, first + stride, ... < end of the selection's global (kGlobal) or rank-local part: exchanged
+// global cells go to sink(i, val, cnt), all others straight into the results.
+template <bool kGlobal, class Sink>
+__device__ __forceinline__ void finalize(const Selection &S, uint64_t *acc, long long *cnt, const uint32_t *desc, bool reset,
+                                         bool exchange, const Results &out, int first, int end, int stride, Sink sink) {
+    for (int i = first; i < end; i += stride) {
+        const int cell = kGlobal ? S.glob_cell(i) : S.loc_cell(i);
+        uint64_t val;
+        long long n;
+        finalize_cell(acc, cnt, desc[cell], cell, val, n, reset);
+        if constexpr (kGlobal) {
+            if (exchange) {
+                sink(i, val, n);
+                continue;
+            }
+        }
+        out.put(cell, val, n > 0 ? 0 : 1);
+    }
+}
+
+// Header check of ranks first, first + stride, ... < world before any record index is trusted: OK, or LAYOUT when a
+// rank's header(r) differs from ours.  The hash covers the globally-reduced cells (names, shapes, ops, cell ranges); the
+// rank-local tail of the selection may legitimately differ between ranks.
+template <class Header>
+__device__ __forceinline__ int check_headers(int first, int world, int stride, uint64_t hash, int n_glob, Header header) {
+    int st = DMLB_METRIC_OK;
+    for (int r = first; r < world; r += stride) {
+        const Record h = header(r);
+        if (h.v != hash || h.n != (uint64_t)n_glob) st = DMLB_METRIC_LAYOUT;
+    }
+    return st;
+}
+
+// Combine global selection indices first, first + stride, ... < end in rank order into the results: fetch(i) makes
+// index i's records readable (false: a peer never delivered them -> TIMEOUT), rec(i, r) reads rank r's.
+template <class Fetch, class Rec>
+__device__ __forceinline__ void combine_global(const Selection &S, const uint32_t *desc, int world, const Results &out,
+                                               int first, int end, int stride, int &st, Fetch fetch, Rec rec) {
+    for (int i = first; i < end; i += stride) {
+        if (!fetch(i)) {
+            st = DMLB_METRIC_TIMEOUT;
+            break;
+        }
+        const int cell = S.glob_cell(i);
+        uint64_t v;
+        uint8_t flag;
+        combine_cell(desc[cell], world, [&](int r) { return rec(i, r); }, v, flag, st);
+        out.put(cell, v, flag);
+    }
+}
+
+// The block's status, TIMEOUT > LAYOUT > SPLIT_VOTE > OK over every thread's `st`.  Every thread must call.
+__device__ __forceinline__ int block_worst_status(int st) {
+    if (__syncthreads_or(st == DMLB_METRIC_TIMEOUT)) return DMLB_METRIC_TIMEOUT;
+    if (__syncthreads_or(st == DMLB_METRIC_LAYOUT)) return DMLB_METRIC_LAYOUT;
+    if (__syncthreads_or(st == DMLB_METRIC_SPLIT_VOTE)) return DMLB_METRIC_SPLIT_VOTE;
+    return DMLB_METRIC_OK;
 }
 
 }  // namespace dmlb

@@ -221,132 +221,68 @@ __device__ __noinline__ void metric_cta(const CommDev &c, uint32_t s, const dmlb
     }
     __syncthreads();  // entries may target cells the finalisation below reads (same CTA: block-level ordering is enough)
 
-    // 2. finalise
-    unsigned char *slot = M.out_ring + (size_t)(count % (unsigned long long)M.ring_slots) *
-                                           ((size_t)DMLB_METRIC_STATUS_SLOTS * 4 + 9 * (size_t)M.capacity);
-    int *status = reinterpret_cast<int *>(slot);
-    uint64_t *out_val = reinterpret_cast<uint64_t *>(slot + DMLB_METRIC_STATUS_SLOTS * 4);
-    uint8_t *out_flag = slot + DMLB_METRIC_STATUS_SLOTS * 4 + 8 * (size_t)M.capacity;
-    int n_glob = 0, n_all = 0;
-    for (int j = 0; j < M.n_ranges; ++j) {
-        const int len = M.ranges[j].end - M.ranges[j].begin;
-        n_all += len;
-        if (j < M.n_global_ranges) n_glob += len;
-    }
-    const dmlb_range *lr = M.ranges + M.n_global_ranges;
-    for (int i = threadIdx.x; i < n_all - n_glob; i += kCommThreads) {
-        const int cell = sel_to_cell(lr, M.n_ranges - M.n_global_ranges, i);
-        uint64_t val;
-        long long n;
-        finalize_cell(M.acc, cnt, M.desc[cell], cell, val, n, false);
-        out_val[cell] = val;
-        out_flag[cell] = n > 0 ? 0 : 1;
-    }
-    uint64_t *rec_mine = reinterpret_cast<uint64_t *>(c.mstage(c.rank, half));
-    for (int i = threadIdx.x; i < n_glob; i += kCommThreads) {
-        const int cell = sel_to_cell(M.ranges, M.n_global_ranges, i);
-        uint64_t val;
-        long long n;
-        finalize_cell(M.acc, cnt, M.desc[cell], cell, val, n, false);
-        if (exchange && kLL) {
+    // 2. finalise (no reset)
+    const Results out = Results::block(M.out_ring + (size_t)(count % (unsigned long long)M.ring_slots) * Results::bytes(M.capacity),
+                                       M.capacity);
+    const Selection S = count_selection(M.ranges, M.n_ranges, M.n_global_ranges);
+    uint64_t *mine = reinterpret_cast<uint64_t *>(c.mstage(c.rank, half));
+    // LL record i = lines 2 + 2i (val) and 3 + 2i (cnt) of the source rank's slot; the header is record -1
+    auto ll_put = [&](int dst, int i, uint64_t v, uint64_t n) {
+        uint4 *line = c.ll_metric(dst, half, c.rank) + 2 + 2 * i;
+        ll_store(line, (uint32_t)v, (uint32_t)(v >> 32), s);
+        ll_store(line + 1, (uint32_t)n, (uint32_t)(n >> 32), s);
+    };
+    finalize<false>(S, M.acc, cnt, M.desc, false, false, out, threadIdx.x, S.n_loc, kCommThreads, nullptr);
+    finalize<true>(S, M.acc, cnt, M.desc, false, exchange, out, threadIdx.x, S.n_glob, kCommThreads,
+                   [&](int i, uint64_t v, long long n) {
+                       if (!kLL) return put_record(mine, i, v, (uint64_t)n);
 #pragma unroll
-            for (int r = 0; r < DMLB_MAX_WORLD; ++r)
-                if (r < c.world) {
-                    uint4 *dst = c.ll_metric(r, half, c.rank) + 2 + 2 * i;
-                    ll_store(dst, (uint32_t)val, (uint32_t)(val >> 32), s);
-                    ll_store(dst + 1, (uint32_t)(uint64_t)n, (uint32_t)((uint64_t)n >> 32), s);
-                }
-        } else if (exchange) {
-            rec_mine[2 + 2 * i] = val;
-            rec_mine[3 + 2 * i] = (uint64_t)n;
-        } else {
-            out_val[cell] = val;
-            out_flag[cell] = n > 0 ? 0 : 1;
-        }
-    }
+                       for (int r = 0; r < DMLB_MAX_WORLD; ++r)
+                           if (r < c.world) ll_put(r, i, v, (uint64_t)n);
+                   });
     int st = DMLB_METRIC_OK;
-    if (exchange && kLL) {
-        if (threadIdx.x < c.world) {  // header lines to rank threadIdx.x
-            uint4 *dst = c.ll_metric(threadIdx.x, half, c.rank);
-            ll_store(dst, (uint32_t)M.layout_hash, (uint32_t)(M.layout_hash >> 32), s);
-            ll_store(dst + 1, (uint32_t)n_glob, 0u, s);
-        }
-        // 3. every rank's header has to arrive and agree before any record index is trusted
-        uint4 w[DMLB_MAX_WORLD];
-        bool arrived = true;
-        if (threadIdx.x == 0) {
-            arrived = ll_wait_all(c, s, [&](int r) { return c.ll_metric(c.rank, half, r); }, w);
-            if (arrived) {
-                for (int r = 0; r < c.world; ++r)
-                    if ((((uint64_t)w[r].z << 32) | w[r].x) != M.layout_hash) st = DMLB_METRIC_LAYOUT;
-                arrived = ll_wait_all(c, s, [&](int r) { return c.ll_metric(c.rank, half, r) + 1; }, w);
-                for (int r = 0; arrived && r < c.world; ++r)
-                    if (w[r].x != (uint32_t)n_glob) st = DMLB_METRIC_LAYOUT;
-            }
-            if (!arrived) st = DMLB_METRIC_TIMEOUT;
-        }
-        const bool ok = __syncthreads_or(st != DMLB_METRIC_OK) == 0;
-        // 4. combine in rank order (each thread polls the lines of its own cells)
-        if (ok)
-            for (int i = threadIdx.x; i < n_glob; i += kCommThreads) {
-                const int cell = sel_to_cell(M.ranges, M.n_global_ranges, i);
-                uint4 wv[DMLB_MAX_WORLD], wn[DMLB_MAX_WORLD];
-                const bool got = ll_wait_all(c, s, [&](int r) { return c.ll_metric(c.rank, half, r) + 2 + 2 * i; }, wv) &&
-                                 ll_wait_all(c, s, [&](int r) { return c.ll_metric(c.rank, half, r) + 3 + 2 * i; }, wn);
-                if (!got) {
+    if (exchange) {
+        // 3. every rank's header has to arrive and agree before any record index is trusted, then 4. combine in rank order
+        if (kLL) {
+            if (threadIdx.x < c.world) ll_put(threadIdx.x, -1, M.layout_hash, (uint64_t)S.n_glob);
+            uint4 wv[DMLB_MAX_WORLD], wn[DMLB_MAX_WORLD];
+            auto fetch = [&](int i) {  // wait for every rank's lines of record i (no barrier: each thread polls its own)
+                return ll_wait_all(c, s, [&](int r) { return c.ll_metric(c.rank, half, r) + 2 + 2 * i; }, wv) &&
+                       ll_wait_all(c, s, [&](int r) { return c.ll_metric(c.rank, half, r) + 3 + 2 * i; }, wn);
+            };
+            auto rec = [&](int, int r) { return Record{u64_of(wv[r].x, wv[r].z), u64_of(wn[r].x, wn[r].z)}; };
+            if (threadIdx.x == 0) {  // header lines 0 (hash) and 1 (count), each checked as it arrives
+                uint4 w[DMLB_MAX_WORLD];
+                auto word = [&](int r) { return u64_of(w[r].x, w[r].z); };
+                const uint64_t n_glob = (uint64_t)S.n_glob;
+                const bool hash_in = ll_wait_all(c, s, [&](int r) { return c.ll_metric(c.rank, half, r); }, w);
+                if (hash_in)
+                    st = check_headers(0, c.world, 1, M.layout_hash, S.n_glob, [&](int r) { return Record{word(r), n_glob}; });
+                if (!hash_in || !ll_wait_all(c, s, [&](int r) { return c.ll_metric(c.rank, half, r) + 1; }, w))
                     st = DMLB_METRIC_TIMEOUT;
-                    break;
-                }
-                uint64_t out;
-                uint8_t flag;
-                auto rec = [&](int r, uint64_t &v, long long &n) {
-                    v = ((uint64_t)wv[r].z << 32) | wv[r].x;
-                    n = (long long)(((uint64_t)wn[r].z << 32) | wn[r].x);
-                };
-                combine_cell(M.desc[cell], c.world, rec, out, flag, st);
-                out_val[cell] = out;
-                out_flag[cell] = flag;
+                else if (st == DMLB_METRIC_OK)
+                    st = check_headers(0, c.world, 1, M.layout_hash, S.n_glob, [&](int r) { return Record{M.layout_hash, word(r)}; });
             }
-    } else if (exchange) {
-        if (threadIdx.x == 0) {
-            rec_mine[0] = M.layout_hash;
-            rec_mine[1] = (uint64_t)n_glob;
+            if (__syncthreads_or(st != DMLB_METRIC_OK) == 0)
+                combine_global(S, M.desc, c.world, out, threadIdx.x, S.n_glob, kCommThreads, st, fetch, rec);
+        } else {
+            if (threadIdx.x == 0) put_record(mine, -1, M.layout_hash, (uint64_t)S.n_glob);
+            auto rec = [&](int i, int r) { return load_staged(c.mstage(r, half), i); };
+            // the collective's barrier 0 (this CTA owns flag slot blockIdx.x like any data CTA)
+            st = comm_barrier(c, 0, s)
+                     ? check_headers(threadIdx.x, c.world, kCommThreads, M.layout_hash, S.n_glob, [&](int r) { return rec(-1, r); })
+                     : DMLB_METRIC_TIMEOUT;
+            if (__syncthreads_or(st != DMLB_METRIC_OK) == 0)
+                combine_global(S, M.desc, c.world, out, threadIdx.x, S.n_glob, kCommThreads, st, [](int) { return true; }, rec);
         }
-        // 3. the collective's barrier 0 (this CTA owns flag slot blockIdx.x like any data CTA)
-        const bool arrived = comm_barrier(c, 0, s);
-        if (!arrived) st = DMLB_METRIC_TIMEOUT;
-        if (arrived && threadIdx.x < c.world) {
-            uint4 h = ld_coherent_u4(reinterpret_cast<const uint4 *>(c.mstage(threadIdx.x, half)));
-            const uint64_t ph = ((uint64_t)h.y << 32) | h.x, pn = ((uint64_t)h.w << 32) | h.z;
-            if (ph != M.layout_hash || pn != (uint64_t)n_glob) st = DMLB_METRIC_LAYOUT;
-        }
-        const bool ok = __syncthreads_or(st != DMLB_METRIC_OK) == 0;
-        // 4. combine in rank order
-        if (ok)
-            for (int i = threadIdx.x; i < n_glob; i += kCommThreads) {
-                const int cell = sel_to_cell(M.ranges, M.n_global_ranges, i);
-                uint64_t out;
-                uint8_t flag;
-                auto rec = [&](int r, uint64_t &v, long long &n) {
-                    uint4 w = ld_coherent_u4(reinterpret_cast<const uint4 *>(c.mstage(r, half)) + 1 + i);
-                    v = ((uint64_t)w.y << 32) | w.x;
-                    n = (long long)(((uint64_t)w.w << 32) | w.z);
-                };
-                combine_cell(M.desc[cell], c.world, rec, out, flag, st);
-                out_val[cell] = out;
-                out_flag[cell] = flag;
-            }
     }
-    int worst = DMLB_METRIC_OK;
-    if (__syncthreads_or(st == DMLB_METRIC_TIMEOUT)) worst = DMLB_METRIC_TIMEOUT;
-    else if (__syncthreads_or(st == DMLB_METRIC_LAYOUT)) worst = DMLB_METRIC_LAYOUT;
-    else if (__syncthreads_or(st == DMLB_METRIC_SPLIT_VOTE)) worst = DMLB_METRIC_SPLIT_VOTE;
+    const int worst = block_worst_status(st);
     // 5. publish: results first, then the stamp (the host trusts a slot only when its stamp matches)
     __syncthreads();
     if (threadIdx.x == 0) {
-        status[0] = worst;
+        out.status[0] = worst;
         __threadfence_system();
-        *reinterpret_cast<volatile unsigned long long *>(slot + DMLB_METRIC_STATUS_SLOTS * 4 - 8) = count + 1ull;
+        *out.stamp() = count + 1ull;
         *reinterpret_cast<volatile unsigned long long *>(M.counter) = count + 1ull;
     }
 }
@@ -669,16 +605,10 @@ int dmlb_comm_allreduce(void *comm, float *bucket, size_t n, int wire, float sca
         const dmlb_step_metrics &m = *metrics;
         if (!m.acc || !m.cnt || !m.desc || !m.counter || !m.out_ring || m.ring_slots < 1 || m.capacity < 1)
             return DMLB_EINVAL;
-        if (m.n_folds < 0 || m.n_folds > DMLB_MAX_FOLD_ENTRIES || m.n_ranges < 0 || m.n_ranges > DMLB_MAX_RANGES ||
-            m.n_global_ranges < 0 || m.n_global_ranges > m.n_ranges)
-            return DMLB_ECAPACITY;
-        long long n_glob = 0;
-        for (int j = 0; j < m.n_ranges; ++j) {
-            if (m.ranges[j].begin < 0 || m.ranges[j].end < m.ranges[j].begin || m.ranges[j].end > m.n_cells ||
-                m.ranges[j].end > m.capacity)
-                return DMLB_EINVAL;
-            if (j < m.n_global_ranges) n_glob += m.ranges[j].end - m.ranges[j].begin;
-        }
+        if (m.n_folds < 0 || m.n_folds > DMLB_MAX_FOLD_ENTRIES) return DMLB_ECAPACITY;
+        long long n_glob = 0, n_loc = 0;
+        const int rc = check_selection(m.ranges, m.n_ranges, m.n_global_ranges, min(m.n_cells, m.capacity), n_glob, n_loc);
+        if (rc != DMLB_OK) return rc;
         if (n_glob > DMLB_STEP_METRIC_MAX_CELLS) return DMLB_ECAPACITY;
         for (int j = 0; j < m.n_folds; ++j) {
             const dmlb_fold_entry &e = m.folds[j];

@@ -126,6 +126,26 @@ def _world(group=None):
 STATUS_BYTES = 4 * N.METRIC_STATUS_SLOTS  # one int32 status slot per CTA of a reduce launch
 
 
+class ResultBlock:
+    """Result block of capacity C: int32 status[METRIC_STATUS_SLOTS] | u64 val[C] | u8 flag[C] (ring slots: see stamp)."""
+
+    def __init__(self, capacity):
+        self.val, self.flag, self.bytes = (STATUS_BYTES + k * capacity for k in (0, 8, 9))  # byte offsets, size
+        self.stamp = slice(STATUS_BYTES - 8, STATUS_BYTES)  # a step-ring slot: u64 stamp in slots 30-31, status in 0
+
+    def addresses(self, base):  # (status, val, flag) of the block at `base`
+        return base, base + self.val, base + self.flag
+
+    def status(self, block, slots=N.METRIC_STATUS_SLOTS):
+        return block[:STATUS_BYTES].view(torch.int32)[:slots].max()
+
+    def vals(self, block):
+        return block[self.val:self.flag].view(torch.int64)
+
+    def parse(self, block, slots=N.METRIC_STATUS_SLOTS):  # (status, vals, flags) copied out of a uint8 block tensor
+        return int(self.status(block, slots)), self.vals(block).clone(), block[self.flag:self.bytes].clone()
+
+
 class _PendingResult:
     """Results of one reduce launch on their way to the host: the kernel writes them straight into mapped pinned host
     memory (or they are copied there), and an event marks completion.  The block belongs to a small ring owned by the
@@ -141,12 +161,8 @@ class _PendingResult:
     def get(self):
         if self._parsed is None:
             self.event.synchronize()
-            cap = self.capacity
-            status = int(self.host[:STATUS_BYTES].view(torch.int32).max())
-            vals = self.host[STATUS_BYTES:STATUS_BYTES + 8 * cap].view(torch.int64).clone()
-            flags = self.host[STATUS_BYTES + 8 * cap:STATUS_BYTES + 9 * cap].clone()
+            self._parsed = ResultBlock(self.capacity).parse(self.host)
             self.host = None  # the ring slot may be reused from here on
-            self._parsed = (status, vals, flags)
         return self._parsed
 
 
@@ -158,13 +174,12 @@ class StepRing:
     SLOTS = 8
 
     def __init__(self, lib, capacity):
-        self.capacity = capacity
-        self.slot_bytes = STATUS_BYTES + 9 * capacity
-        self.host = torch.zeros(self.SLOTS, self.slot_bytes, dtype=torch.uint8).pin_memory()
+        self.capacity, self.block = capacity, ResultBlock(capacity)
+        self.host = torch.zeros(self.SLOTS, self.block.bytes, dtype=torch.uint8).pin_memory()
         out = ctypes.c_void_p()
         N.check(lib.dmlb_host_device_pointer(self.host.data_ptr(), ctypes.byref(out)), 'host_device_pointer(ring)')
         self.device_ptr = out.value
-        self._stamps = self.host.numpy()[:, STATUS_BYTES - 8:STATUS_BYTES].view('<u8').reshape(self.SLOTS)
+        self._stamps = self.host.numpy()[:, self.block.stamp].view('<u8').reshape(self.SLOTS)
 
     def stamp(self, k):
         return int(self._stamps[(k - 1) % self.SLOTS])
@@ -193,12 +208,7 @@ class StepRing:
                 raise RuntimeError(f'step exchange {k} never reported its results (stamp {got})')
 
     def read(self, k):
-        row = self.host[(k - 1) % self.SLOTS]
-        cap = self.capacity
-        status = int(row[:4].view(torch.int32)[0])
-        vals = row[STATUS_BYTES:STATUS_BYTES + 8 * cap].view(torch.int64).clone()
-        flags = row[STATUS_BYTES + 8 * cap:STATUS_BYTES + 9 * cap].clone()
-        return status, vals, flags
+        return self.block.parse(self.host[(k - 1) % self.SLOTS], slots=1)  # slots 30-31: the stamp
 
 
 class _RingResult:
@@ -336,7 +346,8 @@ class DeviceSlab:
             for k, t in new.items():
                 t[:self.capacity].copy_(getattr(self, k))
         self.acc, self.cnt, self.desc = new['acc'], new['cnt'], new['desc']
-        self.out = torch.zeros(STATUS_BYTES + 9 * capacity, dtype=torch.uint8, device=self.device)
+        self.block = ResultBlock(capacity)
+        self.out = torch.zeros(self.block.bytes, dtype=torch.uint8, device=self.device)
         self.capacity = capacity
         self._ptrs = (self.acc.data_ptr(), self.cnt.data_ptr(), self.desc.data_ptr(), self.out.data_ptr())
         for slot in getattr(self, '_host_pool', []):  # results still sitting in blocks of the old size: read them out
@@ -376,16 +387,9 @@ class DeviceSlab:
         """(pinned host block, device address of it or None, its event).  The blocks form a fixed ring (no allocation and
         no cudaHostAlloc stall in steady state: the p99 of r1's per-step exchange was exactly that); a block whose previous
         result has not been read yet is parsed out first.  Status slots are zero on hand-out."""
-        size = STATUS_BYTES + 9 * self.capacity
-        ring = self._host_pool
-        if not ring or ring[0]['host'].numel() != size:
-            for slot in ring:
-                if slot['pending'] is not None:
-                    slot['pending'].get()
-            ring = self._host_pool = []
-            self._host_next = 0
+        ring = self._host_pool  # (emptied by _grow whenever the block size changes)
         if len(ring) < self.HOST_RING:
-            host = torch.zeros(size, dtype=torch.uint8, pin_memory=True)
+            host = torch.zeros(self.block.bytes, dtype=torch.uint8, pin_memory=True)
             dptr = None
             if self._host_mapped is not False:
                 out = ctypes.c_void_p()
@@ -517,7 +521,7 @@ class DeviceSlab:
             slot = self._acquire_host()
             if slot['dptr'] is not None:
                 base = slot['dptr']  # the kernel writes its results straight into mapped pinned host memory
-        status_ptr, val_ptr, flag_ptr = base, base + STATUS_BYTES, base + STATUS_BYTES + 8 * self.capacity
+        status_ptr, val_ptr, flag_ptr = self.block.addresses(base)
         if base == out_p:  # device-resident block: clear the sticky status slots (ring blocks are handed out zeroed)
             N.check(lib.dmlb_memset_async(status_ptr, 0, STATUS_BYTES, st), 'memset(status)')
 
@@ -557,9 +561,8 @@ class DeviceSlab:
         if base == out_p:  # pinned memory not device-mapped on this platform: one D2H copy instead
             slot['host'].copy_(self.out, non_blocking=True)
         slot['event'].record()
-        pending = _PendingResult(self, slot['host'], slot['event'], self.capacity)
-        slot['pending'] = pending
-        return pending
+        slot['pending'] = _PendingResult(self, slot['host'], slot['event'], self.capacity)
+        return slot['pending']
 
     def _reduce_prepared(self, plan_key, global_ranges, local_ranges, layout_hash, reset, exchange):
         """The per-step hot path of reduce(): the same selection as last time (`plan_key` identifies it), results into
@@ -592,18 +595,17 @@ class DeviceSlab:
             return None
         args = prep['slots'].get(id(slot))
         if args is None:
-            base, acc_p, cnt_p, desc_p = slot['dptr'], self._ptrs[0], self._ptrs[1], self._ptrs[2]
+            status_p, val_p, flag_p = self.block.addresses(slot['dptr'])
             args = prep['slots'][id(slot)] = (
-                prep['comm'], ctypes.c_void_p(acc_p), ctypes.c_void_p(cnt_p), ctypes.c_void_p(desc_p), ctypes.c_int(self.n_cells),
+                prep['comm'], *(ctypes.c_void_p(p) for p in self._ptrs[:3]), ctypes.c_int(self.n_cells),
                 prep['arr'], ctypes.c_int(prep['n']), ctypes.c_int(prep['n_glob']), prep['hash'], ctypes.c_int(int(reset)),
-                ctypes.c_void_p(base + STATUS_BYTES), ctypes.c_void_p(base + STATUS_BYTES + 8 * self.capacity), ctypes.c_void_p(base))
+                ctypes.c_void_p(val_p), ctypes.c_void_p(flag_p), ctypes.c_void_p(status_p))
         rc = self._lib().dmlb_metric_reduce(*args, N.stream_ptr())
         if rc:
             N.check(rc, 'metric_reduce')
         slot['event'].record()
-        pending = _PendingResult(self, slot['host'], slot['event'], self.capacity)
-        slot['pending'] = pending
-        return pending
+        slot['pending'] = _PendingResult(self, slot['host'], slot['event'], self.capacity)
+        return slot['pending']
 
     def _reduce_via_collective(self, lib, ranges, layout_hash, reset, world, rank, val_ptr, flag_ptr, status_ptr, st):
         """Exchange through torch.distributed (NCCL all_gather of the packed record) when no peer arena is attached.
@@ -637,8 +639,7 @@ class DeviceSlab:
 
     def result_view(self, cell, lanes, is_int):
         """Device view of the last reduce's values for cells [cell, cell+lanes) (no host sync)."""
-        vals = self.out[STATUS_BYTES:STATUS_BYTES + 8 * self.capacity].view(torch.int64 if is_int else torch.float64)
-        return vals[cell:cell + lanes]
+        return self.block.vals(self.out).view(torch.int64 if is_int else torch.float64)[cell:cell + lanes]
 
     # -- checkpoint --------------------------------------------------------------------------------------------------
     def export_cells(self, cell, lanes, device_tensors=False):
@@ -706,9 +707,8 @@ def _device_reduce(stacked, reduction, dims, steps_axis, group=None, globally=Fa
     layout = _layout_hash(('reduce', lanes, reduction.value, str(dtype)))
     rng = [(cell, cell + lanes)]
     slab.reduce(rng if globally else [], [] if globally else rng, layout, reset=True, exchange=globally, to_host=False)
-    is_int = not _is_float(dtype)
-    result = slab.result_view(cell, lanes, is_int).to(out_dtype).reshape(residual)
-    status = slab.out[:STATUS_BYTES].view(torch.int32).max().reshape(1)
+    result = slab.result_view(cell, lanes, not _is_float(dtype)).to(out_dtype).reshape(residual)
+    status = slab.block.status(slab.out).reshape(1)
     slab.release_to(mark)
     return result, status
 

@@ -356,7 +356,7 @@ class TestSlabEdgeCases:
         """A reduce may take several launches that share one status block: an error an earlier launch recorded must
         survive a later clean launch (C ABI: finalize -> combine of fabricated 2-rank records)."""
         from dmlcloud_b200 import _native as N
-        from dmlcloud_b200.metrics import STATUS_BYTES, DeviceSlab, Reduction, _desc_word
+        from dmlcloud_b200.metrics import STATUS_BYTES, DeviceSlab, Reduction, ResultBlock, _desc_word
 
         slab = DeviceSlab(torch.device('cuda', 0))
         lib, st = slab._lib(), N.stream_ptr()
@@ -374,18 +374,19 @@ class TestSlabEdgeCases:
         slab.fold_imm(cell, 2.5, False)
         slab.flush()
         full = record()
-        out = torch.zeros(STATUS_BYTES + 9 * slab.capacity, dtype=torch.uint8, device='cuda')
-        base = out.data_ptr()
+        block = ResultBlock(slab.capacity)
+        out = torch.zeros(block.bytes, dtype=torch.uint8, device='cuda')
+        status_p, val_p, flag_p = block.addresses(out.data_ptr())
 
         def combine(a, b):
             gathered = torch.cat([a, b])
             N.check(lib.dmlb_metric_combine(gathered.data_ptr(), 2, 0, slab.desc.data_ptr(), arr, 1,
-                                            base + STATUS_BYTES, base + STATUS_BYTES + 8 * slab.capacity, base, st), 'combine')
+                                            val_p, flag_p, status_p, st), 'combine')
             torch.cuda.synchronize()
-            return int(out[:STATUS_BYTES].view(torch.int32).max())
+            return int(block.status(out))
 
         assert combine(full, full) == N.METRIC_OK
-        assert out[STATUS_BYTES:STATUS_BYTES + 8 * slab.capacity].view(torch.float64)[cell].item() == 5.0
+        assert block.vals(out).view(torch.float64)[cell].item() == 5.0
         assert combine(full, empty) == N.METRIC_SPLIT_VOTE
         assert combine(full, full) == N.METRIC_SPLIT_VOTE  # sticky until the caller clears the block
         out[:STATUS_BYTES].zero_()
@@ -421,7 +422,7 @@ def test_fold_warp_path_every_shape_against_fsum(dtype):
     import math
 
     from dmlcloud_b200 import _native as N
-    from dmlcloud_b200.metrics import STATUS_BYTES
+    from dmlcloud_b200.metrics import STATUS_BYTES, ResultBlock
     from helpers import check_launches, dmlb_launches
 
     lib, st = N.cuda_lib(0), N.stream_ptr()
@@ -445,7 +446,8 @@ def test_fold_warp_path_every_shape_against_fsum(dtype):
     desc = desc.cuda()
     acc = torch.zeros(C, dtype=torch.int64, device='cuda')
     cnt = torch.zeros(C, dtype=torch.int64, device='cuda')
-    out = torch.zeros(STATUS_BYTES + 9 * C, dtype=torch.uint8, device='cuda')
+    block = ResultBlock(C)
+    out = torch.zeros(block.bytes, dtype=torch.uint8, device='cuda')
     srcs = [x.cuda().contiguous() for *_, x in cases]
     entries = [N.FoldEntry(s.data_ptr(), 0, {torch.float32: N.F32, torch.float64: N.F64, torch.float16: N.F16,
                                              torch.bfloat16: N.BF16, torch.int64: N.I64, torch.int32: N.I32,
@@ -460,8 +462,9 @@ def test_fold_warp_path_every_shape_against_fsum(dtype):
             part = entries[i:i + N.MAX_FOLD_ENTRIES]
             N.check(lib.dmlb_metric_fold(acc.data_ptr(), cnt.data_ptr(), desc.data_ptr(),
                                          (N.FoldEntry * len(part))(*part), len(part), st))
+        status_p, val_p, flag_p = block.addresses(base)
         N.check(lib.dmlb_metric_reduce(None, acc.data_ptr(), cnt.data_ptr(), desc.data_ptr(), C, ranges, 1, 0, 0, 1,
-                                       base + STATUS_BYTES, base + STATUS_BYTES + 8 * C, base, st))
+                                       val_p, flag_p, status_p, st))
 
     _, launches = dmlb_launches(run)
     folds = [min(N.MAX_FOLD_ENTRIES, len(entries) - i) for i in range(0, len(entries), N.MAX_FOLD_ENTRIES)]
@@ -469,8 +472,8 @@ def test_fold_warp_path_every_shape_against_fsum(dtype):
                    + [('dmlb::metric_reduce_kernel', -(-C // 256))])
     host = out.cpu()
     assert int(host[:STATUS_BYTES].view(torch.int32).abs().max()) == N.METRIC_OK
-    vals = host[STATUS_BYTES:STATUS_BYTES + 8 * C].view(torch.int64 if is_int else torch.float64).numpy()
-    flags = host[STATUS_BYTES + 8 * C:].numpy()
+    _, vals, flags = block.parse(host)
+    vals, flags = vals.view(torch.int64 if is_int else torch.float64).numpy(), flags.numpy()
     assert (flags == 0).all()
     for c0, k, lanes, steps, op, x in cases:
         xs = x.to(torch.int64 if is_int else torch.float64).numpy()  # exact: every source dtype widens exactly
@@ -583,7 +586,7 @@ def _alternating_layout_worker(rank, world, initfile, outdir, n_iter):
 
     from dmlcloud_b200 import _native as N
     from dmlcloud_b200.gradsync import PeerComm
-    from dmlcloud_b200.metrics import STATUS_BYTES
+    from dmlcloud_b200.metrics import ResultBlock
     from helpers import check_launches, dmlb_launches, rank_device
 
     torch.cuda.set_device(rank_device(rank))
@@ -595,7 +598,8 @@ def _alternating_layout_worker(rank, world, initfile, outdir, n_iter):
     acc = torch.zeros(C, dtype=torch.int64, device=dev)
     cnt = torch.zeros(C, dtype=torch.int64, device=dev)
     N.check(lib.dmlb_metric_reset(acc.data_ptr(), cnt.data_ptr(), desc.data_ptr(), 0, C, st))
-    row = -(-(STATUS_BYTES + 9 * C) // 256) * 256  # every result block 256-byte aligned (values are u64, status i32)
+    block = ResultBlock(C)
+    row = -(-block.bytes // 256) * 256  # every result block 256-byte aligned (values are u64, status i32)
     out = torch.zeros(n_iter + 1, row, dtype=torch.uint8, device=dev)
     layouts = [(1, 0x1111), (2, 0x2222_0000_0002), (3, 0x3333_0000_0000_0003)]
     import struct
@@ -608,8 +612,9 @@ def _alternating_layout_worker(rank, world, initfile, outdir, n_iter):
         N.check(lib.dmlb_metric_fold(acc.data_ptr(), cnt.data_ptr(), desc.data_ptr(), ent, n, st))
         base = out[i].data_ptr()
         rng = (N.Range * 1)(N.Range(0, n))
+        status_p, val_p, flag_p = block.addresses(base)
         N.check(lib.dmlb_metric_reduce(comm.handle, acc.data_ptr(), cnt.data_ptr(), desc.data_ptr(), C, rng, 1, 1, h, 1,
-                                       base + STATUS_BYTES, base + STATUS_BYTES + 8 * C, base, st))
+                                       val_p, flag_p, status_p, st))
 
     for i in range(n_iter):
         one(i)
@@ -623,8 +628,8 @@ def _alternating_layout_worker(rank, world, initfile, outdir, n_iter):
     bad = []
     for i in range(n_iter + 1):
         n = layouts[i % 3][0]
-        status = int(host[i, :STATUS_BYTES].view(torch.int32).max())
-        vals = host[i, STATUS_BYTES:STATUS_BYTES + 8 * C].view(torch.float64)[:n].tolist()
+        status, vals, _ = block.parse(host[i, :block.bytes])
+        vals = vals.view(torch.float64)[:n].tolist()
         want = float(sum((r + 1) * (i + 1) for r in range(world)))
         if status != N.METRIC_OK or vals != [want] * n:
             bad.append((i, status, vals))
