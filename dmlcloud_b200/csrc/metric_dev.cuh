@@ -271,6 +271,15 @@ inline int check_selection(const dmlb_range *r, int n_ranges, int n_global_range
     return DMLB_OK;
 }
 
+// Host side: true when no two of the entries fold into a common cell.  Entries of one launch run concurrently (one CTA
+// or warp each) with plain read-modify-writes of acc / cnt, so two entries on one cell would race.
+inline bool folds_disjoint(const dmlb_fold_entry *e, int n) {
+    for (int i = 0; i < n; ++i)
+        for (int j = 0; j < i; ++j)
+            if (e[i].cell < (long long)e[j].cell + e[j].lanes && e[j].cell < (long long)e[i].cell + e[i].lanes) return false;
+    return true;
+}
+
 // A result block: int32 status[DMLB_METRIC_STATUS_SLOTS] | u64 val[C] | u8 flag[C].  A step-ring slot keeps its stamp in
 // the last 8 status bytes.
 struct Results {

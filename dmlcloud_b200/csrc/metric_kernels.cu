@@ -152,6 +152,7 @@ int dmlb_metric_fold(uint64_t *acc, int64_t *cnt, const uint32_t *desc, const dm
         if (e.src_dtype < DMLB_F32 || e.src_dtype > DMLB_U8) return DMLB_EINVAL;  // (feed entries only exist in the step exchange)
         P.e[i] = e;
     }
+    if (!folds_disjoint(P.e, n_entries)) return DMLB_EINVAL;
     metric_fold_kernel<<<n_entries, kFoldThreads, 0, (cudaStream_t)stream>>>(acc, (long long *)cnt, desc, P);
     return launched();
 }

@@ -155,7 +155,9 @@ __device__ __forceinline__ void pack_range(const float *bucket, uint4 *mine, siz
     }
 }
 
-// out(g) = sum over ranks of stage[r][g] for g in [lo, hi) (index space of the staging buffers, offset `goff`)
+// out(g) = sum over ranks of stage[r][g] for g in [lo, hi) (index space of the staging buffers, offset `goff`).
+// Every rank-ordered sum in this file starts from -0.0f, the IEEE additive identity (-0 + x == x bit for bit, whereas
+// +0 + -0 == +0): an element that is -0.0 on every rank stays -0.0, as in the oracle and torch's all-reduce.
 template <int kWire, int kU, class Sink>
 __device__ __forceinline__ void reduce_range(const CommDev &c, int half, size_t lo, size_t hi, size_t goff, Sink sink) {
     typedef Wire<kWire> W;
@@ -178,7 +180,7 @@ __device__ __forceinline__ void reduce_range(const CommDev &c, int half, size_t 
             if (i < hi) {
                 float acc[E];
 #pragma unroll
-                for (int j = 0; j < E; ++j) acc[j] = 0.0f;
+                for (int j = 0; j < E; ++j) acc[j] = -0.0f;
 #pragma unroll
                 for (int r = 0; r < kMaxW; ++r)
                     if (r < c.world) W::accumulate(acc, w[u][r]);
@@ -317,7 +319,7 @@ allreduce_oneshot_kernel(const __grid_constant__ CommDev c, float *bucket, size_
             load_bucket<E>(bucket, g, n, scale, v);
             const uint4 w = W::pack(v);
 #pragma unroll
-            for (int j = 0; j < E; ++j) acc[j] = 0.0f;
+            for (int j = 0; j < E; ++j) acc[j] = -0.0f;
             W::accumulate(acc, w);
             part += store_bucket<E>(bucket, g, n, acc, want_sumsq);
         }
@@ -388,7 +390,7 @@ allreduce_ll_kernel(const __grid_constant__ CommDev c, float *bucket, size_t n, 
         if (!ok) break;
         float acc[EL];
 #pragma unroll
-        for (int j = 0; j < EL; ++j) acc[j] = 0.0f;
+        for (int j = 0; j < EL; ++j) acc[j] = -0.0f;
 #pragma unroll
         for (int r = 0; r < DMLB_MAX_WORLD; ++r)
             if (r < c.world) {
@@ -506,7 +508,7 @@ allreduce_twoshot_kernel(const __grid_constant__ CommDev c, float *bucket, size_
                 if (q < c.world && g < nvec) {
                     float acc[E];
 #pragma unroll
-                    for (int j = 0; j < E; ++j) acc[j] = 0.0f;
+                    for (int j = 0; j < E; ++j) acc[j] = -0.0f;
                     W::accumulate(acc, w[q]);
                     part += store_bucket<E>(bucket, g, n, acc, want_sumsq);
                 }
@@ -619,6 +621,7 @@ int dmlb_comm_allreduce(void *comm, float *bucket, size_t n, int wire, float sca
                 return DMLB_EINVAL;
             }
         }
+        if (!folds_disjoint(m.folds, m.n_folds)) return DMLB_EINVAL;
     }
     cudaStream_t st = (cudaStream_t)stream;
     const bool nvls = W > 1 && c->dev.mc != nullptr &&

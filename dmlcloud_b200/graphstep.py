@@ -335,6 +335,12 @@ class GraphedTrainStep:
                 room = N.MAX_FOLD_ENTRIES - len(entries)
                 cols = dict(sorted(cols.items())[:max(0, min(N.FEED_WIDTH, room))])
                 self.feed.assign(cols)
+            # the entries of one launch must fold into disjoint cells: a value tracked inside the step for a cell that also
+            # has a feed column (the same metric tracked with python scalars between steps) is folded by a launch of its own
+            clash = [any(e.cell <= c < e.cell + e.lanes for c in self.feed.cols) for e in entries]
+            if any(clash):
+                slab._launch_fold([e for e, x in zip(entries, clash) if x])
+                entries = [e for e, x in zip(entries, clash) if not x]
             for cell, j in self.feed.cols.items():
                 entries.append(N.FoldEntry(None, 0, N.SRC_FEED, cell, 1, j, 1, 0))
         metrics, live_names = self._describe_metrics(entries) if stage.live_metrics_every else (None, {})

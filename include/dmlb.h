@@ -192,6 +192,7 @@ int dmlb_comm_set_multicast(void *comm, void *mc_base);
  *   feed:   device address of a mapped pinned host ring [feed_slots][DMLB_FEED_WIDTH][2] doubles ({value, count} pairs) for
  *           host scalars (e.g. misc/step_time_ms); fold entries with src_dtype == DMLB_SRC_FEED and k = column read slot
  *           (count % feed_slots); their `src` field is ignored.  NULL / 0 when unused.
+ *   folds:  like dmlb_metric_fold's entries, they must target disjoint cells (else DMLB_EINVAL, nothing launched).
  *   counter: device uint64, number of exchanges done through this descriptor (the kernel increments it). */
 typedef struct dmlb_step_metrics dmlb_step_metrics; /* defined below, after the metric slab types */
 
@@ -260,7 +261,10 @@ typedef struct {
 
 /* reset cells [begin, end) to the identity of their reduction, cnt = 0 */
 int dmlb_metric_reset(uint64_t *acc, int64_t *cnt, const uint32_t *desc, int begin, int end, void *stream);
-/* fold up to DMLB_MAX_FOLD_ENTRIES values into the slab in one launch; `entries` is a HOST array (copied by value) */
+/* fold up to DMLB_MAX_FOLD_ENTRIES values into the slab in one launch; `entries` is a HOST array (copied by value).
+ * The entries of one launch run concurrently, so they must target DISJOINT cells ([cell, cell + lanes) ranges that do
+ * not overlap); overlapping entries are refused with DMLB_EINVAL before any launch.  The same holds for the fold
+ * entries of a dmlb_step_metrics descriptor, feed entries included (each covers its one cell). */
 int dmlb_metric_fold(uint64_t *acc, int64_t *cnt, const uint32_t *desc, const dmlb_fold_entry *entries, int n_entries,
                      void *stream);
 

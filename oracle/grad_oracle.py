@@ -35,31 +35,32 @@ def round_bf16(x):
     return bf16_bits_to_f32(f32_to_bf16_bits(x))
 
 
-def scale_f32(local, world):
-    """One rank's bucket fill: grad * fl32(1/W), one fp32 rounding."""
-    inv = np.float32(1.0 / world)
+def scale_f32(local, world, scale=None):
+    """One rank's bucket fill: grad * fl32(scale), one fp32 rounding (scale defaults to 1/W)."""
+    inv = np.float32(1.0 / world if scale is None else scale)
     return (np.asarray(local, dtype=np.float32) * inv).astype(np.float32)
 
 
-def allreduce_f32(locals_):
-    """locals_: [W, N] fp32 local gradients -> [N] averaged gradient, fp32 wire, rank-ordered fp32 sum."""
+def allreduce_f32(locals_, scale=None):
+    """locals_: [W, N] fp32 local gradients -> [N] averaged gradient, fp32 wire, rank-ordered fp32 sum.  scale: the
+    factor every rank applies before the sum (default 1/W; the SyncBN statistics use 1.0)."""
     locals_ = np.asarray(locals_, dtype=np.float32)
     world = locals_.shape[0]
-    acc = scale_f32(locals_[0], world)
+    acc = scale_f32(locals_[0], world, scale)
     for r in range(1, world):
-        acc = (acc + scale_f32(locals_[r], world)).astype(np.float32)
+        acc = (acc + scale_f32(locals_[r], world, scale)).astype(np.float32)
     return acc
 
 
-def allreduce_bf16(locals_, round_result=False):
+def allreduce_bf16(locals_, round_result=False, scale=None):
     """bf16 wire: sum over ranks (fp32 accumulate, rank order) of bf16(grad * 1/W).
 
     round_result=True additionally rounds the sum to bf16 (what the two-shot path's all-gather phase carries)."""
     locals_ = np.asarray(locals_, dtype=np.float32)
     world = locals_.shape[0]
-    acc = round_bf16(scale_f32(locals_[0], world))
+    acc = round_bf16(scale_f32(locals_[0], world, scale))
     for r in range(1, world):
-        acc = (acc + round_bf16(scale_f32(locals_[r], world))).astype(np.float32)
+        acc = (acc + round_bf16(scale_f32(locals_[r], world, scale))).astype(np.float32)
     return round_bf16(acc) if round_result else acc
 
 

@@ -117,3 +117,31 @@ def test_product_refuses_to_compute_without_cuda():
 
     with pytest.raises(RuntimeError, match='CUDA'):
         FlatAdam([torch.nn.Parameter(torch.zeros(3))])
+
+
+def test_overlapping_fold_entries_are_refused_before_any_launch():
+    """The fold entries of one launch run concurrently with plain read-modify-writes of their cells: entries that share
+    a cell are refused with EINVAL by dmlb_metric_fold and by the fused step exchange (feed entries count as cells), and
+    nothing is launched.  Fake, aligned device addresses: the refusal comes before any CUDA call."""
+    lib = N.load()
+    a = ctypes.c_void_p(256)
+    before = N.launch_count()
+    overlapping = [N.FoldEntry(256, 0, N.F32, 4, 3, 1, 1, 0), N.FoldEntry(None, 1, N.F64, 6, 1, 1, 1, 0)]  # cell 6 twice
+    ent = (N.FoldEntry * 2)(*overlapping)
+    assert lib.dmlb_metric_fold(a, a, a, ent, 2, None) == N.EINVAL
+    comm = ctypes.c_void_p()
+    arenas = (ctypes.c_void_p * 1)(256)
+    N.check(lib.dmlb_comm_create(ctypes.byref(comm), 1, 0, arenas, 1024))
+    try:
+        for second in (N.FoldEntry(None, 1, N.F64, 6, 1, 1, 1, 0),       # an immediate inside a device entry's cells
+                       N.FoldEntry(None, 0, N.SRC_FEED, 4, 1, 0, 1, 0),  # a feed column on a device entry's first cell
+                       N.FoldEntry(512, 0, N.I64, 2, 3, 33, 1, 0)):      # two device entries sharing cell 4
+            m = N.StepMetrics()
+            m.acc = m.cnt = m.desc = m.counter = m.out_ring = m.feed = 256
+            m.n_cells, m.capacity, m.ring_slots, m.feed_slots = 16, 16, 8, 64
+            m.folds[0], m.folds[1], m.n_folds = N.FoldEntry(256, 0, N.F32, 4, 3, 1, 1, 0), second, 2
+            m.ranges[0], m.n_ranges, m.n_global_ranges = N.Range(0, 16), 1, 1
+            assert lib.dmlb_comm_allreduce(comm, None, 0, N.WIRE_F32, 1.0, None, 0, ctypes.byref(m), None) == N.EINVAL
+    finally:
+        lib.dmlb_comm_destroy(comm)
+    assert N.launch_count() == before

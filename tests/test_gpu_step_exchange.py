@@ -328,3 +328,68 @@ def test_step_exchange_at_metric_cell_capacity(world, wire, n_grad, algo):
             if w['traced']:
                 assert kernel.startswith(f'dmlb::allreduce_{w["proto"]}_kernel<'), (kernel, w)
             check_launches(launches, [(kernel, w['grid'])])
+
+
+# ----------------------------------------------------------------------------------------------------------------------
+# One metric tracked two ways in the captured step: with python scalars between steps (a host-feed column of the step
+# exchange) and with a tensor inside the step (a device fold entry).  The entries of one launch must target disjoint cells,
+# so the step folds the tensor with a launch of its own; the epoch values must equal the uncaptured run's.
+# ----------------------------------------------------------------------------------------------------------------------
+def _run_two_ways(cuda_graph):
+    from dmlcloud_b200 import TrainValStage
+    from dmlcloud_b200.metrics import Reduction
+    from dmlcloud_b200.optim import FlatAdam
+    from dmlcloud_b200.pipeline import TrainingPipeline
+
+    class Tracking:
+        """A loader that tracks a python scalar for the metric before handing out each batch (between two steps)."""
+
+        def __init__(self, stage, batches):
+            self.stage, self.batches = stage, batches
+
+        def __iter__(self):
+            for i, b in enumerate(self.batches):
+                self.stage.track_reduce('mix', 0.25 * i - 1.0, reduction=Reduction.MEAN, prefixed=False)
+                yield b
+
+    class Stage(TrainValStage):
+        def pre_stage(self):
+            torch.manual_seed(0)
+            g = torch.Generator().manual_seed(3)
+            data = [(torch.randn(16, 8, generator=g), torch.randint(0, 4, (16,), generator=g)) for _ in range(8)]
+            self.pipeline.register_dataset('train', Tracking(self, data), verbose=False)
+            self.pipeline.register_dataset('val', data[:1], verbose=False)
+            model = torch.nn.Linear(8, 4)
+            self.pipeline.register_model('lin', model, verbose=False)
+            self.pipeline.register_optimizer('adam', FlatAdam(model.parameters(), lr=1e-3))
+            self.cuda_graph, self.cuda_graph_warmup, self.live_metrics_every = cuda_graph, 1, 1
+
+        def step(self, batch):
+            x, y = (t.to(self.device) for t in batch)
+            self.track_reduce('mix', y.float().mean(), reduction=Reduction.MEAN, prefixed=False)  # k/16: exact sums
+            return torch.nn.functional.cross_entropy(self.pipeline.models['lin'](x), y)
+
+    p = TrainingPipeline(name='two-ways')
+    stage = Stage()
+    p.append_stage(stage, max_epochs=2)
+    p.run()
+    torch.cuda.synchronize()
+    return p, stage
+
+
+def test_metric_tracked_by_host_scalars_and_in_the_captured_step_matches_eager():
+    from dmlcloud_b200.util.distributed import deinitialize_torch_distributed, init_process_group_dummy
+
+    runs = {}
+    for cuda_graph in (False, True):
+        init_process_group_dummy()
+        try:
+            p, stage = _run_two_ways(cuda_graph)
+            runs[cuda_graph] = ([h.item() for h in p.tracker['mix']], p.tracker['misc/total_train_batches'][-1].item())
+            if cuda_graph:
+                g = stage._graph
+                assert g is not None and g.replays >= 8 and g.step_metrics is not None
+                assert g.feed is not None and g.feed.cols, 'the scalars of the metric take a host-feed column'
+        finally:
+            deinitialize_torch_distributed()
+    assert runs[True] == runs[False], runs
