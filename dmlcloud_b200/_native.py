@@ -72,6 +72,9 @@ SIGNATURES = {
     'dmlb_bucket_round_bf16_f32': (c_int, [c_void_p, c_size_t, c_float, c_void_p, c_void_p]),
     'dmlb_bucket_sumsq_f32': (c_int, [c_void_p, c_size_t, c_void_p, c_void_p]),
     'dmlb_bucket_clip_f32': (c_int, [c_void_p, c_size_t, c_void_p, c_float, c_void_p]),
+    'dmlb_bucket_scale_bf16': (c_int, [c_void_p, c_size_t, c_float, c_void_p]),
+    'dmlb_bucket_sumsq_bf16': (c_int, [c_void_p, c_size_t, c_void_p, c_void_p]),
+    'dmlb_bucket_clip_bf16': (c_int, [c_void_p, c_size_t, c_void_p, c_float, c_void_p]),
     'dmlb_adam_step_f32': (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_size_t, c_double, c_double, c_double,
                                    c_double, c_double, c_int, c_int, c_void_p, c_float, c_void_p, c_int, c_void_p,
                                    c_int, c_void_p]),
@@ -89,6 +92,7 @@ SIGNATURES = {
     'dmlb_comm_set_multicast': (c_int, [c_void_p, c_void_p]),
     'dmlb_comm_allreduce': (c_int, [c_void_p, c_void_p, c_size_t, c_int, c_float, c_void_p, c_int, POINTER(StepMetrics),
                                     c_void_p]),
+    'dmlb_comm_allreduce_bf16': (c_int, [c_void_p, c_void_p, c_size_t, c_float, c_void_p, c_int, c_void_p]),
     'dmlb_vmm_granularity': (c_size_t, [c_int, c_int]),
     'dmlb_vmm_alloc': (c_int, [c_int, c_size_t, POINTER(c_void_p), POINTER(c_int), POINTER(c_uint64)]),
     'dmlb_vmm_import': (c_int, [c_int, c_int, c_size_t, POINTER(c_void_p), POINTER(c_uint64)]),

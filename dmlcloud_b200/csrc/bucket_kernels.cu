@@ -41,7 +41,7 @@ constexpr int kUnroll = 4;      // independent vector loads a thread issues befo
 constexpr int kCtasPerSm = 4;
 
 // Each functor says how many elements one of its vector items covers (4: one 128-bit fp32 access; 8: one 128-bit bf16
-// access = two 128-bit fp32 accesses).
+// access).
 template <class F>
 struct elems_of {
     static constexpr int value = 4;
@@ -184,12 +184,87 @@ struct ClipF32 {  // buf *= min(1, max_norm / (sqrt(*sumsq) + 1e-6))   8 B/elem,
     }
 };
 
-__device__ __forceinline__ void prologue(ClipF32 &f) {
-    // torch.nn.utils.clip_grad_norm_: clip_coef = max_norm / (total_norm + 1e-6), clamped to 1.0, all in fp32
+// ---- bf16 buckets (DDP's bucket of bf16 parameters): one 128-bit access = 8 elements, arithmetic in fp32, stores RNE --
+__device__ __forceinline__ uint32_t scale_bf16x2(uint32_t w, float s) { return pack_bf16x2(bf16_lo(w) * s, bf16_hi(w) * s); }
+__device__ __forceinline__ uint4 scale_bf16x8(uint4 v, float s) {
+    v.x = scale_bf16x2(v.x, s), v.y = scale_bf16x2(v.y, s), v.z = scale_bf16x2(v.z, s), v.w = scale_bf16x2(v.w, s);
+    return v;
+}
+__device__ __forceinline__ double sumsq_bf16x2(uint32_t w) {
+    const double lo = bf16_lo(w), hi = bf16_hi(w);
+    return lo * lo + hi * hi;
+}
+
+struct ScaleBf16Inplace {  // buf = bf16_rn(float(buf) * s)            4 B/elem — the NCCL route's K1 for a bf16 bucket
+    typedef uint4 In;
+    uint16_t *base;
+    uint4 *vec;
+    float s;
+    __device__ __forceinline__ In ld(size_t i) const { return vec[i]; }
+    __device__ __forceinline__ double st(size_t i, In v) const {
+        vec[i] = scale_bf16x8(v, s);
+        return 0.0;
+    }
+    __device__ __forceinline__ double scalar(size_t e) const {
+        base[e] = f32_to_bf16(bf16_to_f32(base[e]) * s);
+        return 0.0;
+    }
+};
+
+struct SumsqBf16 {  // sum float(buf)^2                              2 B/elem
+    typedef uint4 In;
+    const uint16_t *src;
+    const uint4 *vsrc;
+    __device__ __forceinline__ In ld(size_t i) const { return ld_stream_u4(vsrc + i); }
+    __device__ __forceinline__ double st(size_t, In v) const {
+        return sumsq_bf16x2(v.x) + sumsq_bf16x2(v.y) + sumsq_bf16x2(v.z) + sumsq_bf16x2(v.w);
+    }
+    __device__ __forceinline__ double scalar(size_t e) const {
+        const double f = bf16_to_f32(src[e]);
+        return f * f;
+    }
+};
+
+struct ClipBf16 {  // buf = bf16_rn(float(buf) * coef), coef as ClipF32's  4 B/elem
+    typedef uint4 In;
+    uint16_t *base;
+    uint4 *vec;
+    const double *sumsq;
+    float max_norm;
+    float coef;  // filled per thread in the kernel prologue
+    __device__ __forceinline__ In ld(size_t i) const { return vec[i]; }
+    __device__ __forceinline__ double st(size_t i, In v) const {
+        vec[i] = scale_bf16x8(v, coef);
+        return 0.0;
+    }
+    __device__ __forceinline__ double scalar(size_t e) const {
+        base[e] = f32_to_bf16(bf16_to_f32(base[e]) * coef);
+        return 0.0;
+    }
+};
+
+template <>
+struct elems_of<ScaleBf16Inplace> {
+    static constexpr int value = 8;
+};
+template <>
+struct elems_of<SumsqBf16> {
+    static constexpr int value = 8;
+};
+template <>
+struct elems_of<ClipBf16> {
+    static constexpr int value = 8;
+};
+
+// torch.nn.utils.clip_grad_norm_: clip_coef = max_norm / (total_norm + 1e-6), clamped to 1.0, all in fp32
+template <class F>
+__device__ __forceinline__ void clip_prologue(F &f) {
     float total = (float)sqrt(*f.sumsq);
     float c = f.max_norm / (total + 1e-6f);
     f.coef = c > 1.0f ? 1.0f : c;
 }
+__device__ __forceinline__ void prologue(ClipF32 &f) { clip_prologue(f); }
+__device__ __forceinline__ void prologue(ClipBf16 &f) { clip_prologue(f); }
 template <class F>
 __device__ __forceinline__ void prologue(F &) {}
 
@@ -386,6 +461,30 @@ int dmlb_bucket_clip_f32(float *buf, size_t n, const double *sumsq, float max_no
     long head = head_for(buf, 4, 16);
     ClipF32 f{buf, reinterpret_cast<float4 *>(buf + (head > 0 ? head : 0)), sumsq, max_norm, 1.0f};
     return launch_stream<ClipF32, false>(f, head, n, nullptr, (cudaStream_t)stream);
+}
+
+int dmlb_bucket_scale_bf16(uint16_t *buf, size_t n, float scale, void *stream) {
+    if (!buf && n) return DMLB_EINVAL;
+    if ((uintptr_t)buf & 1) return DMLB_EALIGN;
+    long head = head_for(buf, 2, 16);
+    ScaleBf16Inplace f{buf, reinterpret_cast<uint4 *>(buf + head), scale};
+    return launch_stream<ScaleBf16Inplace, false>(f, head, n, nullptr, (cudaStream_t)stream);
+}
+
+int dmlb_bucket_sumsq_bf16(const uint16_t *buf, size_t n, double *sumsq, void *stream) {
+    if ((!buf && n) || !sumsq) return DMLB_EINVAL;
+    if ((uintptr_t)buf & 1) return DMLB_EALIGN;
+    long head = head_for(buf, 2, 16);
+    SumsqBf16 f{buf, reinterpret_cast<const uint4 *>(buf + head)};
+    return launch_stream<SumsqBf16, true>(f, head, n, sumsq, (cudaStream_t)stream);
+}
+
+int dmlb_bucket_clip_bf16(uint16_t *buf, size_t n, const double *sumsq, float max_norm, void *stream) {
+    if ((!buf && n) || !sumsq) return DMLB_EINVAL;
+    if ((uintptr_t)buf & 1) return DMLB_EALIGN;
+    long head = head_for(buf, 2, 16);
+    ClipBf16 f{buf, reinterpret_cast<uint4 *>(buf + head), sumsq, max_norm, 1.0f};
+    return launch_stream<ClipBf16, false>(f, head, n, nullptr, (cudaStream_t)stream);
 }
 
 }  // extern "C"

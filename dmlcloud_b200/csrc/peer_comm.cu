@@ -20,11 +20,16 @@
 // per-step `track_reduce` traffic (stage.py:305-314) and its cross-rank reduction (metrics.py:121-141) cost no launch
 // and no barrier of their own.
 //
+// A bf16 bucket (dmlb_comm_allreduce_bf16: a bf16 model's DDP bucket) runs the same kernels with the bucket's element type
+// as a template parameter, always on the bf16 wire: bf16 load -> fp32 scale -> bf16 wire -> fp32 sum -> bf16 store.
+//
 // Numerics: one-shot / two-shot accumulate in fp32 in rank order 0..W-1 on every rank => results are bit-identical
-// across ranks and equal to oracle/grad_oracle.py allreduce_f32 / allreduce_bf16.  Two-shot and NVLS with the bf16 wire
+// across ranks and equal to oracle/grad_oracle.py allreduce_f32 / allreduce_bf16 (a bf16 bucket: the bf16 rounding of
+// the latter, allreduce_bf16(round_result=True)).  Two-shot and NVLS with the bf16 wire
 // round the sum to bf16 for the all-gather phase (same as an NCCL bf16 all-reduce).  NVLS sums in the switch (fp32
 // accumulation, order fixed by the hardware, identical on all ranks because every rank receives the same broadcast).
 #include <new>
+#include <type_traits>
 
 #include "metric_dev.cuh"
 #include "peer_comm.cuh"
@@ -84,50 +89,106 @@ __device__ __forceinline__ void mc_store(void *mc, uint4 v) {  // one store, del
                  : "memory");
 }
 
-// load kElems fp32 bucket elements of wire vector g (guarded at the ragged end), scaled
-template <int E>
-__device__ __forceinline__ void load_bucket(const float *bucket, size_t g, size_t n, float scale, float *v) {
+// Bucket element types.  An fp32 bucket travels on either wire; a bf16 bucket (what DDP hands over for bf16 parameters)
+// always travels on the bf16 wire, whose 16-byte vector holds the same 8 elements as one 16-byte load of the bucket.
+// Loads widen to fp32; stores round to the bucket's type (RNE) and return the value stored, so that the fused sum of
+// squares is taken over what the bucket holds.
+template <class T>
+constexpr bool kBf16Bucket = std::is_same<T, __nv_bfloat16>::value;
+
+__device__ __forceinline__ float ld_elem(const float *p, size_t e) { return p[e]; }
+__device__ __forceinline__ float ld_elem(const __nv_bfloat16 *p, size_t e) { return __bfloat162float(p[e]); }
+__device__ __forceinline__ float st_elem(float *p, size_t e, float v) {
+    p[e] = v;
+    return v;
+}
+__device__ __forceinline__ float st_elem(__nv_bfloat16 *p, size_t e, float v) {
+    const __nv_bfloat16 b = __float2bfloat16_rn(v);
+    p[e] = b;
+    return __bfloat162float(b);
+}
+__device__ __forceinline__ void poison_elem(float *p, size_t e) { p[e] = __int_as_float(0x7fc00000); }
+__device__ __forceinline__ void poison_elem(__nv_bfloat16 *p, size_t e) { p[e] = __ushort_as_bfloat16(0x7fc0); }
+
+// load E bucket elements of wire vector g (guarded at the ragged end), scaled
+template <int E, class T>
+__device__ __forceinline__ void load_bucket(const T *bucket, size_t g, size_t n, float scale, float *v) {
     const size_t e0 = g * E;
     if (e0 + E <= n) {
+        if constexpr (kBf16Bucket<T>) {
+            static_assert(E % 8 == 0, "a bf16 bucket travels on the bf16 wire");
 #pragma unroll
-        for (int j = 0; j < E; j += 4) {
-            float4 t = *reinterpret_cast<const float4 *>(bucket + e0 + j);
-            v[j] = t.x * scale, v[j + 1] = t.y * scale, v[j + 2] = t.z * scale, v[j + 3] = t.w * scale;
+            for (int j = 0; j < E; j += 8) {
+                const uint4 t = *reinterpret_cast<const uint4 *>(bucket + e0 + j);
+                v[j] = bf16_lo(t.x) * scale, v[j + 1] = bf16_hi(t.x) * scale;
+                v[j + 2] = bf16_lo(t.y) * scale, v[j + 3] = bf16_hi(t.y) * scale;
+                v[j + 4] = bf16_lo(t.z) * scale, v[j + 5] = bf16_hi(t.z) * scale;
+                v[j + 6] = bf16_lo(t.w) * scale, v[j + 7] = bf16_hi(t.w) * scale;
+            }
+        } else {
+#pragma unroll
+            for (int j = 0; j < E; j += 4) {
+                float4 t = *reinterpret_cast<const float4 *>(bucket + e0 + j);
+                v[j] = t.x * scale, v[j + 1] = t.y * scale, v[j + 2] = t.z * scale, v[j + 3] = t.w * scale;
+            }
         }
     } else {
 #pragma unroll
-        for (int j = 0; j < E; ++j) v[j] = (e0 + j < n) ? bucket[e0 + j] * scale : 0.0f;
+        for (int j = 0; j < E; ++j) v[j] = (e0 + j < n) ? ld_elem(bucket, e0 + j) * scale : 0.0f;
     }
 }
 
-template <int E>
-__device__ __forceinline__ double store_bucket(float *bucket, size_t g, size_t n, const float *v, bool sumsq) {
+template <int E, class T>
+__device__ __forceinline__ double store_bucket(T *bucket, size_t g, size_t n, const float *v, bool sumsq) {
     const size_t e0 = g * E;
     double p = 0.0;
     if (e0 + E <= n) {
+        if constexpr (kBf16Bucket<T>) {
 #pragma unroll
-        for (int j = 0; j < E; j += 4)
-            *reinterpret_cast<float4 *>(bucket + e0 + j) = make_float4(v[j], v[j + 1], v[j + 2], v[j + 3]);
-        if (sumsq) {
+            for (int j = 0; j < E; j += 8) {
+                uint4 o;
+                o.x = pack_bf16x2(v[j], v[j + 1]), o.y = pack_bf16x2(v[j + 2], v[j + 3]);
+                o.z = pack_bf16x2(v[j + 4], v[j + 5]), o.w = pack_bf16x2(v[j + 6], v[j + 7]);
+                *reinterpret_cast<uint4 *>(bucket + e0 + j) = o;
+                if (sumsq) {
+                    const uint32_t w[4] = {o.x, o.y, o.z, o.w};
 #pragma unroll
-            for (int j = 0; j < E; ++j) p += (double)v[j] * v[j];
+                    for (int k = 0; k < 4; ++k) {
+                        const float lo = bf16_lo(w[k]), hi = bf16_hi(w[k]);
+                        p += (double)lo * lo;
+                        p += (double)hi * hi;
+                    }
+                }
+            }
+        } else {
+#pragma unroll
+            for (int j = 0; j < E; j += 4)
+                *reinterpret_cast<float4 *>(bucket + e0 + j) = make_float4(v[j], v[j + 1], v[j + 2], v[j + 3]);
+            if (sumsq) {
+#pragma unroll
+                for (int j = 0; j < E; ++j) p += (double)v[j] * v[j];
+            }
         }
     } else {
 #pragma unroll
         for (int j = 0; j < E; ++j)
             if (e0 + j < n) {
-                bucket[e0 + j] = v[j];
-                if (sumsq) p += (double)v[j] * v[j];
+                if constexpr (kBf16Bucket<T>) {
+                    const float s = st_elem(bucket, e0 + j, v[j]);
+                    if (sumsq) p += (double)s * s;
+                } else {  // (spelled out: through st_elem the fp32 kernels compile to other code)
+                    bucket[e0 + j] = v[j];
+                    if (sumsq) p += (double)v[j] * v[j];
+                }
             }
     }
     return p;
 }
 
 // A peer did not arrive: overwrite this CTA's part of the bucket with NaN so that nobody trains on a partial sum.
-template <int E>
-__device__ __forceinline__ void poison_range(float *bucket, size_t lo, size_t hi, size_t n) {
-    const float nan = __int_as_float(0x7fc00000);
-    for (size_t e = lo * E + threadIdx.x; e < hi * E && e < n; e += kCommThreads) bucket[e] = nan;
+template <int E, class T>
+__device__ __forceinline__ void poison_range(T *bucket, size_t lo, size_t hi, size_t n) {
+    for (size_t e = lo * E + threadIdx.x; e < hi * E && e < n; e += kCommThreads) poison_elem(bucket, e);
 }
 
 // ---------------------------------------------------------------------------------------------------------------------
@@ -136,8 +197,8 @@ __device__ __forceinline__ void poison_range(float *bucket, size_t lo, size_t hi
 // kU vectors x W ranks into registers before the first add (kU = 4 for W <= 2, 2 for W <= 4, 1 for W <= 8 keeps the
 // register budget at ~32 data registers).
 // ---------------------------------------------------------------------------------------------------------------------
-template <int kWire, int kU>
-__device__ __forceinline__ void pack_range(const float *bucket, uint4 *mine, size_t lo, size_t hi, size_t n, float scale) {
+template <int kWire, int kU, class T>
+__device__ __forceinline__ void pack_range(const T *bucket, uint4 *mine, size_t lo, size_t hi, size_t n, float scale) {
     typedef Wire<kWire> W;
     constexpr int E = W::kElems;
     for (size_t g0 = lo + threadIdx.x; g0 < hi; g0 += (size_t)kCommThreads * kU) {
@@ -292,9 +353,9 @@ __device__ __noinline__ void metric_cta(const CommDev &c, uint32_t s, const dmlb
 // ---------------------------------------------------------------------------------------------------------------------
 // one-shot
 // ---------------------------------------------------------------------------------------------------------------------
-template <int kWire, int kU>
+template <class T, int kWire, int kU>
 __global__ void __launch_bounds__(kCommThreads, 2)
-allreduce_oneshot_kernel(const __grid_constant__ CommDev c, float *bucket, size_t n, size_t nvec, float scale,
+allreduce_oneshot_kernel(const __grid_constant__ CommDev c, T *bucket, size_t n, size_t nvec, float scale,
                          double *sumsq_out, int n_data, const __grid_constant__ dmlb_step_metrics M) {
     typedef Wire<kWire> W;
     constexpr int E = W::kElems;
@@ -347,9 +408,9 @@ allreduce_oneshot_kernel(const __grid_constant__ CommDev c, float *bucket, size_
 // then polls its own arena's lines of the same indices from all W sources and sums in rank order — bit-identical to the
 // barrier one-shot and to the oracle.
 // ---------------------------------------------------------------------------------------------------------------------
-template <int kWire>
+template <class T, int kWire>
 __global__ void __launch_bounds__(kCommThreads, 2)
-allreduce_ll_kernel(const __grid_constant__ CommDev c, float *bucket, size_t n, size_t n_lines, float scale,
+allreduce_ll_kernel(const __grid_constant__ CommDev c, T *bucket, size_t n, size_t n_lines, float scale,
                     double *sumsq_out, int n_data, const __grid_constant__ dmlb_step_metrics M) {
     constexpr int EL = kWire == DMLB_WIRE_BF16 ? 4 : 2;  // elements per line
     const uint32_t s = comm_begin(c);
@@ -367,7 +428,7 @@ allreduce_ll_kernel(const __grid_constant__ CommDev c, float *bucket, size_t n, 
         float v[EL];
         const size_t e0 = l * EL;
 #pragma unroll
-        for (int j = 0; j < EL; ++j) v[j] = (e0 + j < n) ? bucket[e0 + j] * scale : 0.0f;
+        for (int j = 0; j < EL; ++j) v[j] = (e0 + j < n) ? ld_elem(bucket, e0 + j) * scale : 0.0f;
         uint32_t d0, d1;
         if (kWire == DMLB_WIRE_BF16) {
             d0 = pack_bf16x2(v[0], v[1]);
@@ -405,13 +466,12 @@ allreduce_ll_kernel(const __grid_constant__ CommDev c, float *bucket, size_t n, 
 #pragma unroll
         for (int j = 0; j < EL; ++j)
             if (e0 + j < n) {
-                bucket[e0 + j] = acc[j];
-                if (want_sumsq) part += (double)acc[j] * acc[j];
+                const float stored = st_elem(bucket, e0 + j, acc[j]);
+                if (want_sumsq) part += (double)stored * stored;
             }
     }
     if (__syncthreads_or(!ok)) {  // a peer died: nobody trains on a partial sum
-        const float nan = __int_as_float(0x7fc00000);
-        for (size_t e = lo * EL + threadIdx.x; e < hi * EL && e < n; e += kCommThreads) bucket[e] = nan;
+        for (size_t e = lo * EL + threadIdx.x; e < hi * EL && e < n; e += kCommThreads) poison_elem(bucket, e);
         part = __longlong_as_double(0x7ff8000000000000ll);
     }
     if (sumsq_out) {
@@ -430,9 +490,9 @@ allreduce_ll_kernel(const __grid_constant__ CommDev c, float *bucket, size_t n, 
 // kNvls = 2: only the reduce-scatter goes through the switch (one request stream per GPU instead of W-1); the reduced slices
 // stay in their owner's result half and the all-gather is the peer-load phase of the plain two-shot, fused with K2.
 // ---------------------------------------------------------------------------------------------------------------------
-template <int kWire, int kU, int kNvls>
+template <class T, int kWire, int kU, int kNvls>
 __global__ void __launch_bounds__(kCommThreads, 2)
-allreduce_twoshot_kernel(const __grid_constant__ CommDev c, float *bucket, size_t n, size_t nvec, size_t S, float scale,
+allreduce_twoshot_kernel(const __grid_constant__ CommDev c, T *bucket, size_t n, size_t nvec, size_t S, float scale,
                          double *sumsq_out, int n_data, const __grid_constant__ dmlb_step_metrics M) {
     typedef Wire<kWire> W;
     constexpr int E = W::kElems;
@@ -540,6 +600,78 @@ constexpr size_t kNvlsMinBytes = 8 << 20;
 constexpr int kNvlsMinWorld = 8;
 static_assert(sizeof(dmlb_step_metrics) == 1880, "dmlb_step_metrics layout (dmlcloud_b200/_native.py StepMetrics mirrors it)");
 
+// The launch half of dmlb_comm_allreduce / dmlb_comm_allreduce_bf16 (arguments already checked).  T = float: the wire is
+// the caller's; T = __nv_bfloat16: always the bf16 wire.
+template <class T>
+static int allreduce_launch(Comm *c, T *bucket, size_t n, int wire, float scale, double *sumsq, int algo,
+                            const dmlb_step_metrics *metrics, cudaStream_t st) {
+    constexpr bool kF32Bucket = std::is_same<T, float>::value;
+    static_assert(kF32Bucket || kBf16Bucket<T>, "bucket element type");
+    const int W = c->dev.world;
+    const int E = wire == DMLB_WIRE_BF16 ? 8 : 4;
+    const size_t nvec = (n + E - 1) / E;
+    const size_t bytes = nvec * 16;
+    static const dmlb_step_metrics kNoMetrics = {};
+    const bool nvls = W > 1 && c->dev.mc != nullptr &&
+                      (algo == 3 || algo == 4 || (algo == 0 && W >= kNvlsMinWorld && bytes >= kNvlsMinBytes));
+    if ((algo == 3 || algo == 4) && !nvls && W > 1) return DMLB_ESTATE;
+    const bool nvls_rs_only = nvls && algo == 4;
+    const bool oneshot = !nvls && (W == 1 || algo == 1 || algo == 5 || (algo == 0 && (bytes <= kOneshotMaxBytes || W <= 2)));
+    // small messages at W > 1: the LL protocol (no barrier, no peer loads); algo 5 forces the barrier one-shot for A/B runs
+    if (oneshot && W > 1 && algo != 5 && bytes <= kLLMaxPayload) {
+        const int EL = wire == DMLB_WIRE_BF16 ? 4 : 2;
+        const size_t n_lines = (n + EL - 1) / EL;
+        size_t want = (n_lines + kCommThreads - 1) / kCommThreads;  // one line per thread while the grid can grow
+        const size_t cap = (size_t)min(kMaxCtas, sm_count() * 2) - 1;
+        if (want > cap) want = cap;
+        const int n_data = n == 0 ? 0 : (int)(want < 1 ? 1 : want);
+        const int grid = n_data + (metrics ? 1 : 0);
+        const dmlb_step_metrics &Mll = metrics ? *metrics : kNoMetrics;
+        if (wire == DMLB_WIRE_BF16)
+            allreduce_ll_kernel<T, DMLB_WIRE_BF16><<<grid, kCommThreads, 0, st>>>(c->dev, bucket, n, n_lines, scale, sumsq,
+                                                                                  n_data, Mll);
+        else if constexpr (kF32Bucket)
+            allreduce_ll_kernel<T, DMLB_WIRE_F32><<<grid, kCommThreads, 0, st>>>(c->dev, bucket, n, n_lines, scale, sumsq,
+                                                                                 n_data, Mll);
+        return launched();
+    }
+    const int kU = W <= 2 ? 4 : (W <= 4 ? 2 : 1);
+    const size_t items = oneshot ? nvec : (nvec + W - 1) / W;  // vectors a CTA grid is spread over
+    size_t want = (items + (size_t)kCommThreads * kU - 1) / ((size_t)kCommThreads * kU);
+    // all CTAs co-resident (the per-CTA barriers need that); one slot is kept for the metric CTA
+    size_t cap = (size_t)min(kMaxCtas, sm_count() * 2) - 1;
+    if (want > cap) want = cap;
+    const int n_data = n == 0 ? 0 : (int)(want < 1 ? 1 : want);
+    const int grid = n_data + (metrics ? 1 : 0);
+    const dmlb_step_metrics &M = metrics ? *metrics : kNoMetrics;
+#define DMLB_LAUNCH_AR(WIRE, U)                                                                                          \
+    do {                                                                                                                 \
+        if (oneshot)                                                                                                     \
+            allreduce_oneshot_kernel<T, WIRE, U><<<grid, kCommThreads, 0, st>>>(c->dev, bucket, n, nvec, scale, sumsq,   \
+                                                                                n_data, M);                              \
+        else if (nvls_rs_only)                                                                                           \
+            allreduce_twoshot_kernel<T, WIRE, U, 2><<<grid, kCommThreads, 0, st>>>(c->dev, bucket, n, nvec, items,     \
+                                                                                   scale, sumsq, n_data, M);             \
+        else if (nvls)                                                                                                   \
+            allreduce_twoshot_kernel<T, WIRE, U, 1><<<grid, kCommThreads, 0, st>>>(c->dev, bucket, n, nvec, items,     \
+                                                                                   scale, sumsq, n_data, M);             \
+        else                                                                                                             \
+            allreduce_twoshot_kernel<T, WIRE, U, 0><<<grid, kCommThreads, 0, st>>>(c->dev, bucket, n, nvec, items,     \
+                                                                                   scale, sumsq, n_data, M);             \
+    } while (0)
+    if (wire == DMLB_WIRE_BF16) {
+        if (kU == 4) DMLB_LAUNCH_AR(DMLB_WIRE_BF16, 4);
+        else if (kU == 2) DMLB_LAUNCH_AR(DMLB_WIRE_BF16, 2);
+        else DMLB_LAUNCH_AR(DMLB_WIRE_BF16, 1);
+    } else if constexpr (kF32Bucket) {
+        if (kU == 4) DMLB_LAUNCH_AR(DMLB_WIRE_F32, 4);
+        else if (kU == 2) DMLB_LAUNCH_AR(DMLB_WIRE_F32, 2);
+        else DMLB_LAUNCH_AR(DMLB_WIRE_F32, 1);
+    }
+#undef DMLB_LAUNCH_AR
+    return launched();
+}
+
 }  // namespace dmlb
 
 using namespace dmlb;
@@ -597,12 +729,9 @@ int dmlb_comm_allreduce(void *comm, float *bucket, size_t n, int wire, float sca
     if ((uintptr_t)bucket & 15) return DMLB_EALIGN;
     if (n == 0 && !metrics) return DMLB_OK;
     Comm *c = reinterpret_cast<Comm *>(comm);
-    const int W = c->dev.world;
     const int E = wire == DMLB_WIRE_BF16 ? 8 : 4;
-    const size_t nvec = (n + E - 1) / E;
-    const size_t bytes = nvec * 16;
-    if (W > 1 && bytes > c->dev.msg_cap) return DMLB_ECAPACITY;
-    static const dmlb_step_metrics kNoMetrics = {};
+    const size_t bytes = (n + E - 1) / E * 16;
+    if (c->dev.world > 1 && bytes > c->dev.msg_cap) return DMLB_ECAPACITY;
     if (metrics) {
         const dmlb_step_metrics &m = *metrics;
         if (!m.acc || !m.cnt || !m.desc || !m.counter || !m.out_ring || m.ring_slots < 1 || m.capacity < 1)
@@ -623,63 +752,17 @@ int dmlb_comm_allreduce(void *comm, float *bucket, size_t n, int wire, float sca
         }
         if (!folds_disjoint(m.folds, m.n_folds)) return DMLB_EINVAL;
     }
-    cudaStream_t st = (cudaStream_t)stream;
-    const bool nvls = W > 1 && c->dev.mc != nullptr &&
-                      (algo == 3 || algo == 4 || (algo == 0 && W >= kNvlsMinWorld && bytes >= kNvlsMinBytes));
-    if ((algo == 3 || algo == 4) && !nvls && W > 1) return DMLB_ESTATE;
-    const bool nvls_rs_only = nvls && algo == 4;
-    const bool oneshot = !nvls && (W == 1 || algo == 1 || algo == 5 || (algo == 0 && (bytes <= kOneshotMaxBytes || W <= 2)));
-    // small messages at W > 1: the LL protocol (no barrier, no peer loads); algo 5 forces the barrier one-shot for A/B runs
-    if (oneshot && W > 1 && algo != 5 && bytes <= kLLMaxPayload) {
-        const int EL = wire == DMLB_WIRE_BF16 ? 4 : 2;
-        const size_t n_lines = (n + EL - 1) / EL;
-        size_t want = (n_lines + kCommThreads - 1) / kCommThreads;  // one line per thread while the grid can grow
-        const size_t cap = (size_t)min(kMaxCtas, sm_count() * 2) - 1;
-        if (want > cap) want = cap;
-        const int n_data = n == 0 ? 0 : (int)(want < 1 ? 1 : want);
-        const int grid = n_data + (metrics ? 1 : 0);
-        const dmlb_step_metrics &Mll = metrics ? *metrics : kNoMetrics;
-        if (wire == DMLB_WIRE_BF16)
-            allreduce_ll_kernel<DMLB_WIRE_BF16><<<grid, kCommThreads, 0, st>>>(c->dev, bucket, n, n_lines, scale, sumsq, n_data, Mll);
-        else
-            allreduce_ll_kernel<DMLB_WIRE_F32><<<grid, kCommThreads, 0, st>>>(c->dev, bucket, n, n_lines, scale, sumsq, n_data, Mll);
-        return launched();
-    }
-    const int kU = W <= 2 ? 4 : (W <= 4 ? 2 : 1);
-    const size_t items = oneshot ? nvec : (nvec + W - 1) / W;  // vectors a CTA grid is spread over
-    size_t want = (items + (size_t)kCommThreads * kU - 1) / ((size_t)kCommThreads * kU);
-    // all CTAs co-resident (the per-CTA barriers need that); one slot is kept for the metric CTA
-    size_t cap = (size_t)min(kMaxCtas, sm_count() * 2) - 1;
-    if (want > cap) want = cap;
-    const int n_data = n == 0 ? 0 : (int)(want < 1 ? 1 : want);
-    const int grid = n_data + (metrics ? 1 : 0);
-    const dmlb_step_metrics &M = metrics ? *metrics : kNoMetrics;
-#define DMLB_LAUNCH_AR(WIRE, U)                                                                                          \
-    do {                                                                                                                 \
-        if (oneshot)                                                                                                     \
-            allreduce_oneshot_kernel<WIRE, U><<<grid, kCommThreads, 0, st>>>(c->dev, bucket, n, nvec, scale, sumsq,      \
-                                                                             n_data, M);                                 \
-        else if (nvls_rs_only)                                                                                           \
-            allreduce_twoshot_kernel<WIRE, U, 2><<<grid, kCommThreads, 0, st>>>(c->dev, bucket, n, nvec, items, scale,   \
-                                                                                sumsq, n_data, M);                       \
-        else if (nvls)                                                                                                   \
-            allreduce_twoshot_kernel<WIRE, U, 1><<<grid, kCommThreads, 0, st>>>(c->dev, bucket, n, nvec, items, scale,   \
-                                                                                sumsq, n_data, M);                       \
-        else                                                                                                             \
-            allreduce_twoshot_kernel<WIRE, U, 0><<<grid, kCommThreads, 0, st>>>(c->dev, bucket, n, nvec, items, scale,   \
-                                                                                sumsq, n_data, M);                       \
-    } while (0)
-    if (wire == DMLB_WIRE_BF16) {
-        if (kU == 4) DMLB_LAUNCH_AR(DMLB_WIRE_BF16, 4);
-        else if (kU == 2) DMLB_LAUNCH_AR(DMLB_WIRE_BF16, 2);
-        else DMLB_LAUNCH_AR(DMLB_WIRE_BF16, 1);
-    } else {
-        if (kU == 4) DMLB_LAUNCH_AR(DMLB_WIRE_F32, 4);
-        else if (kU == 2) DMLB_LAUNCH_AR(DMLB_WIRE_F32, 2);
-        else DMLB_LAUNCH_AR(DMLB_WIRE_F32, 1);
-    }
-#undef DMLB_LAUNCH_AR
-    return launched();
+    return allreduce_launch(c, bucket, n, wire, scale, sumsq, algo, metrics, (cudaStream_t)stream);
+}
+
+int dmlb_comm_allreduce_bf16(void *comm, uint16_t *bucket, size_t n, float scale, double *sumsq, int algo, void *stream) {
+    if (!comm || (!bucket && n)) return DMLB_EINVAL;
+    if ((uintptr_t)bucket & 15) return DMLB_EALIGN;
+    if (n == 0) return DMLB_OK;
+    Comm *c = reinterpret_cast<Comm *>(comm);
+    if (c->dev.world > 1 && (n + 7) / 8 * 16 > c->dev.msg_cap) return DMLB_ECAPACITY;
+    return allreduce_launch(c, reinterpret_cast<__nv_bfloat16 *>(bucket), n, DMLB_WIRE_BF16, scale, sumsq, algo, nullptr,
+                            (cudaStream_t)stream);
 }
 
 int dmlb_comm_error(void *comm, int *error) {

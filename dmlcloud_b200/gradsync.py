@@ -12,6 +12,9 @@ Per bucket it picks one of three routes, all of them running libdmlb kernels on 
          sum of all W stagings -> write-back into the fp32 bucket (+ optional sum of squares).  No NCCL.
   nccl   K1 (scale / scale+cast to bf16) -> torch.distributed all_reduce (NCCL over NVLink) -> K2 (bf16 -> fp32)
   single W == 1: K1/K2 only (the cast round-trip still happens for the bf16 wire so numerics do not depend on W)
+
+A bf16 bucket (DDP's bucket of bf16 parameters) is already in wire format: it always travels as bf16, whatever `wire`
+says, through the same three routes (dmlb_comm_allreduce_bf16 / dmlb_bucket_scale_bf16 + all_reduce / in place).
 """
 import ctypes
 import warnings
@@ -385,7 +388,7 @@ class GradBucketSync:
         return self.reduce_bucket(buf, bucket.index())
 
     def reduce_bucket(self, buf, index=0):
-        """Average the flat fp32 gradient bucket `buf` across ranks in place; returns a Future of `buf`."""
+        """Average the flat fp32 or bf16 gradient bucket `buf` across ranks in place; returns a Future of `buf`."""
         if not self.profile_events:
             return self._reduce_bucket(buf, index)
         # CUDA events on the stream the kernels are launched on (torch.cuda.Event only sees torch's current stream;
@@ -402,8 +405,11 @@ class GradBucketSync:
         return fut
 
     def _reduce_bucket(self, buf, index=0):
-        if buf.dtype != torch.float32 or not buf.is_contiguous():
-            raise RuntimeError('GradBucketSync expects contiguous fp32 gradient buckets')
+        if buf.dtype not in (torch.float32, torch.bfloat16) or not buf.is_contiguous():
+            raise RuntimeError(f'GradBucketSync expects contiguous fp32 or bf16 gradient buckets, got a '
+                               f'{"" if buf.is_contiguous() else "non-contiguous "}{buf.dtype} bucket')
+        if buf.dtype == torch.bfloat16:
+            return self._reduce_bucket_bf16(buf, index)
         lib = N.cuda_lib(self.device.index)  # runs on the autograd thread: per-thread device of libdmlb's runtime
         n = buf.numel()
         wire = WIRES[self.wire]
@@ -462,6 +468,45 @@ class GradBucketSync:
 
         return fut.then(finish_bf16)
 
+    def _reduce_bucket_bf16(self, buf, index):
+        """A bf16 bucket: bf16 wire always (it is the bucket's own format; `self.wire` governs fp32 buckets only).
+        Result = bf16_rn(sum over ranks, fp32 in rank order, of bf16_rn(g_r * 1/W)); sumsq over the stored bf16 values."""
+        lib = N.cuda_lib(self.device.index)
+        n = buf.numel()
+        sumsq_ptr = self.sumsq.data_ptr() if self.sumsq is not None else None
+        self.buckets_seen += 1
+        self.buckets_this_step += 1
+
+        if self.world == 1:  # the average of one rank is the bucket itself (1/W = 1 multiplies exactly)
+            if sumsq_ptr:
+                N.check(lib.dmlb_bucket_sumsq_bf16(buf.data_ptr(), n, sumsq_ptr, N.stream_ptr()), 'sumsq_bf16')
+            self.last_routes[index] = 'single'
+            return self._done(buf)
+
+        if self.comm is not None and self.comm.fits(((n + 7) // 8) * 16) and buf.data_ptr() % 16 == 0:
+            self.comm_stream.wait_stream(torch.cuda.current_stream(self.device))
+            with torch.cuda.stream(self.comm_stream):
+                N.check(lib.dmlb_comm_allreduce_bf16(self.comm.handle, buf.data_ptr(), n, self.scale, sumsq_ptr,
+                                                     self.algo, N.stream_ptr(self.comm_stream)), 'comm_allreduce_bf16')
+                buf.record_stream(self.comm_stream)
+                fut = self._done(buf)
+            self.last_routes[index] = 'peer'
+            return fut
+
+        # NCCL route: scale in place -> all_reduce (bf16) -> sum of squares of the result
+        self.last_routes[index] = 'nccl'
+        N.check(lib.dmlb_bucket_scale_bf16(buf.data_ptr(), n, self.scale, N.stream_ptr()), 'scale_bf16')
+        fut = dist.all_reduce(buf, group=self.group, async_op=True).get_future()
+
+        def finish(f):
+            out = f.value()[0]
+            if sumsq_ptr:
+                N.check(N.cuda_lib(self.device.index).dmlb_bucket_sumsq_bf16(out.data_ptr(), n, sumsq_ptr,
+                                                                              N.stream_ptr()), 'sumsq_bf16')
+            return out
+
+        return fut.then(finish)
+
     def close(self):
         if self.comm is not None:
             self.comm.close()
@@ -471,9 +516,11 @@ class GradBucketSync:
 def clip_grad_norm_(parameters, max_norm, sumsq=None):
     """torch.nn.utils.clip_grad_norm_ (reference stage.py:276-279) on libdmlb kernels, without a host sync:
     sum of squares (fp64 partials) -> coefficient computed on the device -> in-place scale.
+    fp32 and bf16 gradients (mixed in one list) share one fp64 sum and one fp32 coefficient; a bf16 gradient is
+    rescaled as bf16_rn(g * coef).
     If `sumsq` (a 1-element fp64 CUDA tensor already holding sum g^2 of exactly these parameters, e.g. accumulated by the
     fused all-reduce) is given, the first pass is skipped.  Returns the 0-d CUDA tensor holding the total norm."""
-    grads = [p.grad for p in parameters if p.grad is not None]
+    grads = [_flat(p.grad) for p in parameters if p.grad is not None]
     if not grads:
         return torch.tensor(0.0)
     device = grads[0].device
@@ -482,14 +529,20 @@ def clip_grad_norm_(parameters, max_norm, sumsq=None):
     if sumsq is None:
         sumsq = torch.zeros(1, dtype=torch.float64, device=device)
         for g in grads:
-            N.check(lib.dmlb_bucket_sumsq_f32(_flat_f32(g).data_ptr(), g.numel(), sumsq.data_ptr(), st), 'sumsq')
+            if g.dtype == torch.bfloat16:
+                N.check(lib.dmlb_bucket_sumsq_bf16(g.data_ptr(), g.numel(), sumsq.data_ptr(), st), 'sumsq_bf16')
+            else:
+                N.check(lib.dmlb_bucket_sumsq_f32(g.data_ptr(), g.numel(), sumsq.data_ptr(), st), 'sumsq')
     for g in grads:
-        N.check(lib.dmlb_bucket_clip_f32(_flat_f32(g).data_ptr(), g.numel(), sumsq.data_ptr(), float(max_norm), st),
-                'clip')
+        if g.dtype == torch.bfloat16:
+            N.check(lib.dmlb_bucket_clip_bf16(g.data_ptr(), g.numel(), sumsq.data_ptr(), float(max_norm), st),
+                    'clip_bf16')
+        else:
+            N.check(lib.dmlb_bucket_clip_f32(g.data_ptr(), g.numel(), sumsq.data_ptr(), float(max_norm), st), 'clip')
     return sumsq.sqrt().to(torch.float32).reshape(())
 
 
-def _flat_f32(g):
-    if g.dtype != torch.float32 or not g.is_contiguous():
-        raise RuntimeError('clip_grad_norm_ (dmlcloud_b200) expects contiguous fp32 gradients')
+def _flat(g):
+    if g.dtype not in (torch.float32, torch.bfloat16) or not g.is_contiguous():
+        raise RuntimeError('clip_grad_norm_ (dmlcloud_b200) expects contiguous fp32 or bf16 gradients')
     return g

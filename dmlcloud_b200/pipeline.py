@@ -114,7 +114,10 @@ class TrainingPipeline:
             lines = [f'Model "{name}":', f'    - Parameters: {n_params / 1e6:.1f} kk', f'    - DDP: {use_ddp}']
             if sync is not None:
                 route = 'fused NVLink peer kernel' if sync.comm else ('NCCL' if sync.world > 1 else 'single GPU')
-                lines.append(f'    - Gradient exchange: {sync.wire} wire, {route}')
+                wire = f'{sync.wire} wire'
+                if any(p.dtype == torch.bfloat16 for p in model.parameters()):
+                    wire += ' for fp32 buckets, bf16 buckets travel as bf16'
+                lines.append(f'    - Gradient exchange: {wire}, {route}')
             self.logger.info('\n'.join(lines + [f'    - {model}']))
 
     def _convert_sync_bn(self, model):

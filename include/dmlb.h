@@ -105,6 +105,21 @@ int dmlb_bucket_sumsq_f32(const float *buf, size_t n, double *sumsq, void *strea
 /* buf *= min(1, max_norm / (sqrt(*sumsq) + 1e-6))  — second half of clip_grad_norm_; reads *sumsq on device, no host sync */
 int dmlb_bucket_clip_f32(float *buf, size_t n, const double *sumsq, float max_norm, void *stream);
 
+/* bf16 buckets: what DDP hands the comm hook for bf16 parameters (a model cast with .to(torch.bfloat16), or the bf16
+ * layers of a mixed model).  `buf` holds bf16 bit patterns and needs 2-byte alignment (a scalar head reaches 16 bytes).
+ * Arithmetic in fp32, every store rounded to bf16 (RNE).  Algorithmic bytes/element: scale 4, sumsq 2, clip 4.
+ *   buf = bf16_rn(float(buf) * scale): the rank's share, bf16(grad * (1/W)) as torch's Reducer fills a bf16 bucket
+ *   (reducer.cpp mark_variable_ready_dense, behind reference pipeline.py:74); the NCCL route's step before all_reduce. */
+int dmlb_bucket_scale_bf16(uint16_t *buf, size_t n, float scale, void *stream);
+/* sum(float(buf)^2) in fp64 added to *sumsq: the first half of clip_grad_norm_ (reference stage.py:276-279) over the
+ * bf16 values the bucket stores */
+int dmlb_bucket_sumsq_bf16(const uint16_t *buf, size_t n, double *sumsq, void *stream);
+/* buf = bf16_rn(float(buf) * coef), coef = min(1, max_norm / (sqrt(*sumsq) + 1e-6)) in fp32 exactly as
+ * dmlb_bucket_clip_f32 computes it: the second half of clip_grad_norm_ (reference stage.py:276-279).  torch rounds the
+ * per-tensor norms, the total and the coefficient to bf16 instead; the two rules differ by a few bf16 ulps per element
+ * (DESIGN.md §3). */
+int dmlb_bucket_clip_bf16(uint16_t *buf, size_t n, const double *sumsq, float max_norm, void *stream);
+
 /* ------------------------------------------------------------------------------------------------------------------ */
 /* K5: optimizer step on a flat fp32 bucket (SURVEY §8 f-4)                                                            */
 /* ------------------------------------------------------------------------------------------------------------------ */
@@ -208,6 +223,17 @@ typedef struct dmlb_step_metrics dmlb_step_metrics; /* defined below, after the 
  * dtype in place), so numerics and launch structure do not depend on W. */
 int dmlb_comm_allreduce(void *comm, float *bucket, size_t n, int wire, float scale, double *sumsq, int algo,
                         const dmlb_step_metrics *metrics, void *stream);
+/* in-place averaged all-reduce of a bf16 bucket (bf16 bit patterns), replacing the same allreduce(SUM) of reference
+ * pipeline.py:74 for a bf16 model.  A bf16 bucket always travels on the bf16 wire (16 B = 8 elements, the same vector as
+ * the bucket's own), so it costs 2 B/element of HBM each way and the same NVLink bytes as dmlb_comm_allreduce with
+ * DMLB_WIRE_BF16; the kernels, protocols, grids and `algo` values are that call's.
+ *   bucket = bf16_rn( sum_r float(bf16_rn(float(bucket_r) * scale)) ), fp32 sum in rank order from -0.0 — bit-identical
+ *   on every rank for algo 0, 1, 2 and 5 (one-shot, LL and two-shot give the same bits); NVLS within one bf16 ulp.
+ * sumsq (optional) receives the fp64 sum of the squared bf16 values stored.  No metrics descriptor: the fused step
+ * exchange belongs to the captured step's fp32 flat bucket.  Errors as dmlb_comm_allreduce: DMLB_EINVAL, DMLB_EALIGN
+ * when bucket is not 16-byte aligned, DMLB_ECAPACITY (nothing launched) when ceil(n / 8) * 16 bytes exceed the arena's
+ * message size at world > 1. */
+int dmlb_comm_allreduce_bf16(void *comm, uint16_t *bucket, size_t n, float scale, double *sumsq, int algo, void *stream);
 /* one flag barrier across all ranks on `stream` (setup / tests) */
 int dmlb_comm_barrier(void *comm, void *stream);
 /* *error != 0 after a peer failed to arrive at a barrier within the timeout.  Blocking 4-byte device read; the host
