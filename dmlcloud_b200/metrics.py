@@ -17,9 +17,11 @@ the arithmetic happens:
                                                             gradient all-reduce kernel (StepRing / HostFeed below)
 
 Host-side cost is part of the path: python scalars for one cell are combined on the host and travel as one immediate, a
-step's device values ride in ONE fold launch (`DeviceSlab.batching`), a reduce of the same selection reuses prepared launch
-arguments (`_reduce_prepared`), results land in a fixed ring of device-mapped pinned blocks (no copy, no allocation), and
-selections / plans are cached across epochs (`_reduce_all_fast`, `live_selection`).
+step's device values ride in ONE fold launch (`DeviceSlab.batching`), and results land in a fixed ring of device-mapped
+pinned blocks (no copy, no allocation).  Every reduce of a tracker (`reduce_all`, `next_epoch`, `reduce_live`, the
+captured step's exchange) goes through one selection plan (`_Plan`) per prefix, metric set and set of prefixes this
+epoch has closed: it is made once and reused across epochs, and it keeps the cell ranges, the layout hash and the
+launch arguments the slab prepares for it.
 
 No CPU path exists for reduced metrics: without CUDA (or without libdmlb.so) tracking a reduced metric raises.
 """
@@ -90,6 +92,15 @@ def _normalize_dims(dim, ndim):
     if len(set(out)) != len(out):
         raise RuntimeError('dim appears multiple times in the list of dims')
     return out
+
+
+def _reducer_dim(reduction, dim):
+    """A reducer's `dim` as a list (None: all dims), after refusing an unknown `reduction` (reference metrics.py:44-155)."""
+    if reduction not in [Reduction.MEAN, Reduction.SUM, Reduction.MIN, Reduction.MAX]:
+        raise ValueError(f'Unknown reduction {reduction}')
+    if isinstance(dim, int):
+        return [dim]
+    return list(dim) if dim is not None else None
 
 
 def _lanes_k(shape, dims):
@@ -294,6 +305,13 @@ class HostFeed:
         return out
 
 
+def _imm_entry(cell, value, is_int, count):
+    """Fold entry of `count` host scalars of one cell, combined on the host into `value`: the immediate is the int value
+    itself or the bits of the fp64 value."""
+    bits = value if is_int else struct.unpack('<q', struct.pack('<d', value))[0]
+    return N.FoldEntry(None, bits, N.F64, cell, 1, 1, count, 0)
+
+
 class DeviceSlab:
     """HBM layout: acc u64[C] | cnt i64[C] | desc u32[C]  +  out = status(32 x i32) | val u64[C] | flag u8[C].
     Results destined for the host are written by the reduce kernel directly into device-mapped pinned host memory
@@ -321,13 +339,11 @@ class DeviceSlab:
         self.acc = self.cnt = self.desc = self.out = None
         self._host_pool = []  # ring of pinned result blocks (see _acquire_host)
         self._host_next = 0
-        self._prepared = {}   # prepared argument sets of the per-step reduce (see _reduce_prepared)
         self._wr = None
-        self._range_cache = {}
         self._host_mapped = None  # None = not probed yet; False = pinned memory is not device-mapped here (copy path)
         self._imm = []           # queued fold entries (immediates, and device values while batching)
         self._imm_cells = set()  # cells the queue touches (an entry per cell per launch: folds are not atomic)
-        self._imm_index = {}     # cell -> position of its queued immediate (python scalars of one cell are pre-combined)
+        self._imm_index = {}     # cell -> (position, value) of its queued immediate (python scalars of one cell are pre-combined)
         self._keep = []          # tensors the queued device entries read
         self.batching = False    # True: device values are queued too and ride in ONE launch per step (stage.py)
         self.feed = None         # HostFeed of a captured step: python scalars of its cells go there instead of a launch
@@ -418,19 +434,20 @@ class DeviceSlab:
         if feed is not None and cell in feed.cols:
             feed.put(cell, value)
             return
-        at = self._imm_index.get(cell)
-        if at is not None:
-            e = self._imm[at]
-            old = e.imm if is_int else struct.unpack('<d', struct.pack('<q', e.imm))[0]
-            new = min(old, value) if op == N.MIN else (max(old, value) if op == N.MAX else old + value)
-            e.imm = new if is_int else struct.unpack('<q', struct.pack('<d', new))[0]
-            e.steps += 1
+        queued = self._imm_index.get(cell)
+        if queued is None:
+            self._queue_imm(cell, value, is_int, 1)
             return
+        at, old = queued
+        new = min(old, value) if op == N.MIN else (max(old, value) if op == N.MAX else old + value)
+        self._imm[at] = _imm_entry(cell, new, is_int, self._imm[at].steps + 1)
+        self._imm_index[cell] = (at, new)
+
+    def _queue_imm(self, cell, value, is_int, count):
         if cell in self._imm_cells or len(self._imm) >= N.MAX_FOLD_ENTRIES:
             self.flush()
-        bits = value if is_int else struct.unpack('<q', struct.pack('<d', value))[0]
-        self._imm_index[cell] = len(self._imm)
-        self._imm.append(N.FoldEntry(None, bits, N.F64, cell, 1, 1, 1, 0))
+        self._imm_index[cell] = (len(self._imm), value)
+        self._imm.append(_imm_entry(cell, value, is_int, count))
         self._imm_cells.add(cell)
 
     def fold_device(self, cell, lanes, k, tensor, steps=1):
@@ -466,12 +483,7 @@ class DeviceSlab:
         (reduce / reset / export / end of a stage)."""
         if self.feed is not None:
             for cell, value, count in self.feed.drain():
-                op, is_int = self.feed.kind[cell]
-                bits = value if is_int else struct.unpack('<q', struct.pack('<d', value))[0]
-                if cell in self._imm_cells or len(self._imm) >= N.MAX_FOLD_ENTRIES:
-                    self.flush()
-                self._imm.append(N.FoldEntry(None, bits, N.F64, cell, 1, 1, count, 0))
-                self._imm_cells.add(cell)
+                self._queue_imm(cell, value, self.feed.kind[cell][1], count)
         self.flush()
 
     def _launch_fold(self, entries):
@@ -490,122 +502,81 @@ class DeviceSlab:
             wr = self._wr = (w, r, self.group)
         return wr[0], wr[1]
 
-    def _range_array(self, ranges):
-        key = tuple(ranges)
-        hit = self._range_cache.get(key)
-        if hit is None:
-            if len(self._range_cache) > 64:
-                self._range_cache.clear()
-            hit = ((N.Range * max(len(key), 1))(*[N.Range(b, e) for b, e in key]), len(key))
-            self._range_cache[key] = hit
-        return hit
-
-    def reduce(self, global_ranges, local_ranges, layout_hash, reset=True, exchange=True, to_host=True, plan_key=None):
+    def reduce(self, global_ranges, local_ranges, layout_hash, reset=True, exchange=True, to_host=True, launches=None):
         """Finalise + cross-rank combine.  `global_ranges` are the cells of globally-reduced metrics (identical layout
         on every rank, covered by `layout_hash`, exchanged); `local_ranges` are rank-local metrics (never exchanged,
-        may differ between ranks).  Returns a _PendingResult (to_host) or None."""
+        may differ between ranks).  `launches`: a dict kept with a selection that is reduced again and again (a
+        MetricTracker plan); the launch arguments prepared for it are cached there.  Returns a _PendingResult (to_host)
+        or None."""
         self.flush_all()
-        if to_host and plan_key is not None:
-            fast = self._reduce_prepared(plan_key, global_ranges, local_ranges, layout_hash, reset, exchange)
-            if fast is not None:
-                return fast
         lib = self._lib()
         world, rank = self._world_rank()
         if not exchange:
             world = 1
         st = N.stream_ptr()
-        slot = None
-        acc_p, cnt_p, desc_p, out_p = self._ptrs
-        base = out_p
-        if to_host:
-            slot = self._acquire_host()
-            if slot['dptr'] is not None:
-                base = slot['dptr']  # the kernel writes its results straight into mapped pinned host memory
+        slot = self._acquire_host() if to_host else None
+        mapped = slot is not None and slot['dptr'] is not None
+        base = slot['dptr'] if mapped else self._ptrs[3]  # mapped: the kernel writes straight into pinned host memory
         status_ptr, val_ptr, flag_ptr = self.block.addresses(base)
-        if base == out_p:  # device-resident block: clear the sticky status slots (ring blocks are handed out zeroed)
+        if not mapped:  # device-resident block: clear the sticky status slots (ring blocks are handed out zeroed)
             N.check(lib.dmlb_memset_async(status_ptr, 0, STATUS_BYTES, st), 'memset(status)')
-
-        def launch(comm_handle, glob, loc):
-            # the exchanged (global) ranges must fit ONE launch: every rank has to issue the same number of collectives
-            if len(glob) > N.MAX_RANGES:
-                raise RuntimeError(f'the globally-reduced metric selection is fragmented into {len(glob)} cell ranges '
-                                   f'(max {N.MAX_RANGES} per exchange)')
-            room = N.MAX_RANGES - len(glob)
-            first = True
-            rest = list(loc)
-            while first or rest:
-                part, rest = rest[:room], rest[room:]
-                g = glob if first else []
-                arr, n = self._range_array(tuple(g) + tuple(part))
-                handle = comm_handle if first else None  # rank-local leftovers never touch the communicator
-                if n or handle is not None:
-                    rc = lib.dmlb_metric_reduce(handle, acc_p, cnt_p, desc_p, self.n_cells, arr, n, len(g), layout_hash,
-                                                int(reset), val_ptr, flag_ptr, status_ptr, st)
-                    if rc:
-                        N.check(rc, 'metric_reduce')
-                first = False
-                room = N.MAX_RANGES
-
-        if world == 1:
-            launch(None, [], list(global_ranges) + list(local_ranges))
-        elif self.comm is not None:
-            # fused path: global cells are exchanged (their record index must agree across ranks), rank-local cells are not
-            launch(self.comm.handle, list(global_ranges), list(local_ranges))
-        else:
-            if local_ranges:
-                launch(None, [], list(local_ranges))
+        for args in self._reduce_args({} if launches is None else launches, global_ranges, local_ranges, layout_hash,
+                                      reset, world, base):
+            rc = lib.dmlb_metric_reduce(*args, st)
+            if rc:
+                N.check(rc, 'metric_reduce')
+        if world > 1 and self.comm is None:
             self._reduce_via_collective(lib, list(global_ranges), layout_hash, reset, world, rank, val_ptr, flag_ptr,
                                         status_ptr, st)
         if not to_host:
             return None
-        if base == out_p:  # pinned memory not device-mapped on this platform: one D2H copy instead
+        if not mapped:  # pinned memory not device-mapped on this platform: one D2H copy instead
             slot['host'].copy_(self.out, non_blocking=True)
         slot['event'].record()
         slot['pending'] = _PendingResult(self, slot['host'], slot['event'], self.capacity)
         return slot['pending']
 
-    def _reduce_prepared(self, plan_key, global_ranges, local_ranges, layout_hash, reset, exchange):
-        """The per-step hot path of reduce(): the same selection as last time (`plan_key` identifies it), results into
-        mapped host memory, one launch.  Everything that does not change between calls — the range array, the ctypes
-        argument objects for each of the ring's result blocks — is prepared once; a call is then: pick the ring slot,
-        clear its 128 status bytes, one foreign call, one event record.  (The per-call Python around the launch was what
-        `reduce_live()` spent most of its time on.)  None -> take the general path."""
-        world, _ = self._world_rank()
-        if not exchange:
-            world = 1
-        if world > 1 and self.comm is None:
-            return None
-        key = (plan_key, bool(reset), world, self.generation, self.n_cells)
-        prep = self._prepared.get(key)
-        if prep is not None and (prep['g'] is not global_ranges or prep['l'] is not local_ranges):
-            prep = None  # an id() collision with a plan that has died: prepare again
+    def _reduce_args(self, launches, global_ranges, local_ranges, layout_hash, reset, world, base):
+        """Argument tuples of the dmlb_metric_reduce calls of one reduce into the result block at `base`.  The range
+        arrays are built once per (slab, generation, cell count, reset, world, communicator) and the ctypes tuples once
+        per result block on top, so a repeated reduce makes no Python objects per call beyond the launch itself."""
+        key = (self, self.generation, self.n_cells, reset, world, self.comm)
+        prep = launches.get(key)
         if prep is None:
-            glob = list(global_ranges) if world > 1 else []
-            loc = list(local_ranges) if world > 1 else list(global_ranges) + list(local_ranges)
-            if len(glob) + len(loc) > N.MAX_RANGES or not (glob or loc):
-                return None
-            if len(self._prepared) > 32:
-                self._prepared.clear()
-            arr, n = self._range_array(tuple(glob) + tuple(loc))
-            prep = self._prepared[key] = {'g': global_ranges, 'l': local_ranges, 'arr': arr, 'n': n, 'n_glob': len(glob), 'slots': {},
-                                          'hash': ctypes.c_uint64(layout_hash),
-                                          'comm': self.comm.handle if world > 1 else None}
-        slot = self._acquire_host()
-        if slot['dptr'] is None:
-            return None
-        args = prep['slots'].get(id(slot))
+            prep = launches[key] = {'calls': self._range_calls(global_ranges, local_ranges, world), 'blocks': {}}
+        args = prep['blocks'].get(base)
         if args is None:
-            status_p, val_p, flag_p = self.block.addresses(slot['dptr'])
-            args = prep['slots'][id(slot)] = (
-                prep['comm'], *(ctypes.c_void_p(p) for p in self._ptrs[:3]), ctypes.c_int(self.n_cells),
-                prep['arr'], ctypes.c_int(prep['n']), ctypes.c_int(prep['n_glob']), prep['hash'], ctypes.c_int(int(reset)),
-                ctypes.c_void_p(val_p), ctypes.c_void_p(flag_p), ctypes.c_void_p(status_p))
-        rc = self._lib().dmlb_metric_reduce(*args, N.stream_ptr())
-        if rc:
-            N.check(rc, 'metric_reduce')
-        slot['event'].record()
-        slot['pending'] = _PendingResult(self, slot['host'], slot['event'], self.capacity)
-        return slot['pending']
+            status, val, flag = (ctypes.c_void_p(p) for p in self.block.addresses(base))
+            cells = (*(ctypes.c_void_p(p) for p in self._ptrs[:3]), ctypes.c_int(self.n_cells))
+            tail = (ctypes.c_uint64(layout_hash), ctypes.c_int(int(reset)), val, flag, status)
+            args = prep['blocks'][base] = [(comm, *cells, arr, ctypes.c_int(n), ctypes.c_int(n_glob), *tail)
+                                           for comm, arr, n, n_glob in prep['calls']]
+        return args
+
+    def _range_calls(self, global_ranges, local_ranges, world):
+        """[(communicator handle, range array, #ranges, #exchanged ranges)] of the dmlb_metric_reduce calls of one reduce.
+        Rank-local ranges beyond what fits next to the exchanged ones go into further launches without the communicator."""
+        if world == 1:
+            exchanged, local, comm = [], [*global_ranges, *local_ranges], None
+        elif self.comm is not None:
+            # fused path: global cells are exchanged (their record index must agree across ranks), rank-local cells are not
+            exchanged, local, comm = list(global_ranges), list(local_ranges), self.comm.handle
+        else:  # the global cells go through torch.distributed (_reduce_via_collective)
+            exchanged, local, comm = [], list(local_ranges), None
+        # the exchanged (global) ranges must fit ONE launch: every rank has to issue the same number of collectives
+        if len(exchanged) > N.MAX_RANGES:
+            raise RuntimeError(f'the globally-reduced metric selection is fragmented into {len(exchanged)} cell ranges '
+                               f'(max {N.MAX_RANGES} per exchange)')
+        calls = []
+        while True:
+            room = N.MAX_RANGES - len(exchanged)
+            ranges, local = exchanged + local[:room], local[room:]
+            if ranges or comm is not None:
+                arr = (N.Range * max(len(ranges), 1))(*[N.Range(b, e) for b, e in ranges])
+                calls.append((comm, arr, len(ranges), len(exchanged)))
+            if not local:
+                return calls
+            exchanged, comm = [], None  # rank-local leftovers never touch the communicator
 
     def _reduce_via_collective(self, lib, ranges, layout_hash, reset, world, rank, val_ptr, flag_ptr, status_ptr, st):
         """Exchange through torch.distributed (NCCL all_gather of the packed record) when no peer arena is attached.
@@ -737,17 +708,10 @@ class MetricReducer:
     """
 
     def __init__(self, reduction=Reduction.MEAN, dim=None, globally=True):
-        if reduction not in [Reduction.MEAN, Reduction.SUM, Reduction.MIN, Reduction.MAX]:
-            raise ValueError(f'Unknown reduction {reduction}')
+        self.dim = _reducer_dim(reduction, dim)
         self.values = []
         self.reduction = reduction
         self.globally = globally
-        if isinstance(dim, int):
-            self.dim = [dim]
-        elif dim is not None:
-            self.dim = list(dim)
-        else:
-            self.dim = None
 
     @staticmethod
     def _snapshot(value):
@@ -846,18 +810,11 @@ class SlabMetric:
     of slab cells.  Values are folded on arrival and not retained."""
 
     def __init__(self, tracker, name, reduction=Reduction.MEAN, dim=None, globally=True):
-        if reduction not in [Reduction.MEAN, Reduction.SUM, Reduction.MIN, Reduction.MAX]:
-            raise ValueError(f'Unknown reduction {reduction}')
+        self.dim = _reducer_dim(reduction, dim)
         self._tracker = tracker
         self.name = name
         self.reduction = reduction
         self.globally = globally
-        if isinstance(dim, int):
-            self.dim = [dim]
-        elif dim is not None:
-            self.dim = list(dim)
-        else:
-            self.dim = None
         self.cell = None  # first slab cell; allocated when the first value shows its shape / dtype
         self.lanes = 0
         self.k = 0
@@ -877,8 +834,7 @@ class SlabMetric:
         self.dtype = dtype
         slab = self._tracker._slab_or_create()
         self.cell = slab.alloc(self.lanes, _desc_word(self.reduction, dtype, self.globally))
-        self._tracker._version += 1
-        self._tracker._layout_version += 1
+        self._tracker._layout_changed()
 
     @property
     def is_int(self):
@@ -965,6 +921,48 @@ class _Deferred:
         self.pending, self.metric = pending, metric
 
 
+def _ranges(metrics):
+    ranges = []
+    for m in metrics:
+        if ranges and ranges[-1][1] == m.cell:
+            ranges[-1][1] = m.cell + m.lanes
+        else:
+            ranges.append([m.cell, m.cell + m.lanes])
+    return [tuple(r) for r in ranges]
+
+
+class _Plan:
+    """What a reduce over the metrics under one prefix covers, in registration order:
+      plain     history lists of the plain metrics (whether they have a value is checked per call)
+      done      names of the reduced metrics that already have a value for this epoch
+      bound     [(metric, history)] of the other reduced metrics that own cells; `by_name` maps their names to them
+      unbound   [(metric, history)] of the other reduced metrics, registered but never tracked
+      vote      history of the first globally-reduced unbound metric: it carries the emptiness vote of a rank with no
+                cells (reference 124-128)
+      ranges    (global ranges, local ranges, layout hash) of `bound`: globally-reduced metrics first, they define the
+                cross-rank layout; rank-local metrics (globally=False) follow and are never exchanged
+      launches  launch arguments DeviceSlab.reduce prepares for `ranges`"""
+
+    def __init__(self, tracker, prefix):
+        self.plain, self.done, self.bound, self.unbound = [], [], [], []
+        for name, history in tracker._histories.items():
+            if prefix is not None and not name.startswith(prefix):
+                continue
+            m = tracker.reducers.get(name)
+            if m is None:
+                self.plain.append(history)
+            elif len(history) >= tracker.epoch:
+                self.done.append(name)
+            else:
+                (self.unbound if m.cell is None else self.bound).append((m, history))
+        self.by_name = {m.name: m for m, _ in self.bound}
+        self.vote = next((h for m, h in self.unbound if m.globally), None)
+        glob = [m for m, _ in self.bound if m.globally]
+        loc = [m for m, _ in self.bound if not m.globally]
+        self.ranges = (_ranges(glob), _ranges(loc), _layout_hash([m.layout_item() for m in glob]))
+        self.launches = {}
+
+
 # ----------------------------------------------------------------------------------------------------------------------
 # MetricTracker (reference metrics.py:158-306)
 # ----------------------------------------------------------------------------------------------------------------------
@@ -988,12 +986,12 @@ class MetricTracker:
         self._comm = None
         self._group = None
         self._deferred_slots = []  # (history list, index) of results not yet brought to the host
-        self._version = 0      # bumped whenever the set of reducible cells can have changed
-        self._layout_version = 0  # bumped when metrics are registered / bound to cells / restored (not by reduces)
-        self._reduce_cache = {}   # prefix -> cached selection + plan of reduce_all (see _reduce_all_fast)
-        self._live_full = {}      # prefix -> (layout version, {name: metric}, plan) of a live exchange over everything
-        self._reduced_this_epoch = False  # True once reduce_all() has given some metric its value for this epoch
-        self._live_plan = None  # (version, prefix, epoch) -> cached selection of reduce_live
+        self._layout_version = 0  # bumped when metrics are registered / bound to cells / restored, or histories assigned
+        # Prefixes whose reduce_all() gave some reduced metric its value this epoch, in order.  With the layout version
+        # this tells which reduced metrics have a value, so the two key the plans.  Where it would not (histories
+        # assigned, or the layout changed after a closure) it is replaced by a token no later epoch repeats.
+        self._closed = ()
+        self._plans = {}  # (prefix, layout version, closed) -> _Plan
 
     # -- wiring ------------------------------------------------------------------------------------------------------
     def bind(self, device=None, comm=None, group=None, slab=None):
@@ -1017,6 +1015,12 @@ class MetricTracker:
     def histories(self, value):
         self._histories = value
         self._deferred_slots = []
+        self._layout_changed(histories_assigned=True)
+
+    def _layout_changed(self, histories_assigned=False):
+        self._layout_version += 1
+        if self._closed or histories_assigned:
+            self._closed = (object(),)
 
     def _materialize(self):
         if not self._deferred_slots:
@@ -1101,8 +1105,7 @@ class MetricTracker:
         if dim is not None and reduction is None:
             raise ValueError('If dim is specified, reduction must be specified as well')
         self._histories[name] = [None] * (self.epoch - 1)
-        self._version += 1
-        self._layout_version += 1
+        self._layout_changed()
         if reduction is not None:
             self.reducers[name] = SlabMetric(self, name, reduction=reduction, dim=dim, globally=globally)
 
@@ -1120,152 +1123,65 @@ class MetricTracker:
             self._histories[name].append(value)
 
     # -- reduce ------------------------------------------------------------------------------------------------------
-    def _select(self, prefix, strict):
-        """Metrics a reduce_all(prefix, strict) call covers, in registration order (reference 258-266)."""
-        plain, reduced = [], []
-        for name in self._histories:
-            if prefix is not None and not name.startswith(prefix):
-                continue
-            if self.has_value(name):
-                if strict:
-                    raise ValueError(f'History for {name} has already been reduced for epoch {self.epoch}')
-                continue
-            reducer = self.reducers.get(name)
-            (plain if reducer is None else reduced).append(name)
-        return plain, reduced
-
-    @staticmethod
-    def _ranges(metrics):
-        ranges = []
-        for m in metrics:
-            if ranges and ranges[-1][1] == m.cell:
-                ranges[-1][1] = m.cell + m.lanes
-            else:
-                ranges.append([m.cell, m.cell + m.lanes])
-        return [tuple(r) for r in ranges]
-
-    def _plan(self, bound):
-        """(global ranges, local ranges, layout hash) for a list of cell-owning metrics.  Globally-reduced metrics go
-        first and define the cross-rank layout; rank-local metrics (globally=False) follow and are never exchanged."""
-        glob = [m for m in bound if m.globally]
-        loc = [m for m in bound if not m.globally]
-        return self._ranges(glob), self._ranges(loc), _layout_hash([m.layout_item() for m in glob])
-
-    def _launch(self, bound, reset, plan=None):
-        """One reduce launch for the bound (cell-owning) metrics.  A cached plan (the same tuple object every call) lets
-        the slab reuse its prepared launch arguments."""
-        slab = self._slab_or_create()
-        g, l, layout = plan if plan is not None else self._plan(bound)
-        return slab.reduce(g, l, layout, reset=reset, exchange=True, plan_key=id(plan) if plan is not None else None)
+    def _plan(self, prefix):
+        key = (prefix, self._layout_version, self._closed)
+        plan = self._plans.get(key)
+        if plan is None:
+            if len(self._plans) > 32:
+                self._plans.clear()
+            plan = self._plans[key] = _Plan(self, prefix)
+        return plan
 
     def reduce_all(self, prefix=None, strict=True):
         """Reduces all metrics and appends their reduced values to the history (reference metrics.py:249-273).
         One kernel launch + one small D2H copy for ALL selected metrics, instead of three collectives per metric."""
-        self._reduced_this_epoch = True
-        if self._reduce_all_fast(prefix):
+        plan = self._plan(prefix)
+        epoch = self.epoch
+        if strict and (plan.done or any(len(h) >= epoch for h in plan.plain)):
+            name = next(n for n in self._histories if (prefix is None or n.startswith(prefix)) and self.has_value(n))
+            raise ValueError(f'History for {name} has already been reduced for epoch {epoch}')
+        for h in plan.plain:
+            if len(h) < epoch:
+                h.append(None)
+        if not (plan.bound or plan.unbound):
             return
-        plain, reduced = self._select(prefix, strict)
-        for name in plain:
-            self._histories[name].append(None)
-        if not reduced:
-            return
-        metrics = [self.reducers[name] for name in reduced]
-        bound = [m for m in metrics if m.cell is not None]
-        world, _ = _world(self._group)
         pending = None
         # With W>1 every rank that selected a globally-reduced metric takes part in the exchange, even if it has
         # nothing to contribute: that is how "some workers tracked values and some did not" (reference 124-128) shows.
-        if bound or (world > 1 and any(m.globally for m in metrics)):
-            pending = self._launch(bound, reset=True)
-        vote_carrier = None
-        self._version += 1
-        for m in metrics:
-            if m.cell is None:
-                self._histories[m.name].append(None)
-                if vote_carrier is None and m.globally:
-                    vote_carrier = m
-            else:
-                history = self._histories[m.name]
-                history.append(_Deferred(pending, m))
-                self._deferred_slots.append((history, len(history) - 1))
-            m.count = 0
-        if pending is not None and vote_carrier is not None:
-            history = self._histories[vote_carrier.name]
-            history[-1] = _Deferred(pending, _VoteOnly())
-            self._deferred_slots.append((history, len(history) - 1))
-        if not self.deferred:
-            self._materialize()
-
-    def _reduce_all_fast(self, prefix):
-        """The common epoch end — same metric set as last time, every selected metric owns cells, none has a value for this
-        epoch yet — without the per-metric selection / planning work: the selection, the cell ranges and the layout hash
-        are cached per (layout version, prefix); what remains per metric is one list append.  Returns False when the general path has to run."""
-        cache = self._reduce_cache.get(prefix)
-        if cache is None or cache[0] != self._layout_version:
-            plain = [h for n, h in self._histories.items()
-                     if (prefix is None or n.startswith(prefix)) and n not in self.reducers]
-            pairs = [(self.reducers[n], h) for n, h in self._histories.items()
-                     if (prefix is None or n.startswith(prefix)) and n in self.reducers]
-            if not pairs or any(m.cell is None for m, _ in pairs):
-                return False  # metrics without cells (never tracked): vote-carrier logic of the general path
-            cache = (self._layout_version, plain, pairs, self._plan([m for m, _ in pairs]))
-            if len(self._reduce_cache) > 16:
-                self._reduce_cache.clear()
-            self._reduce_cache[prefix] = cache
-        _, plain, pairs, plan = cache
-        epoch = self.epoch
-        for h in plain:
-            if len(h) >= epoch:
-                return False
-        for _, h in pairs:
-            if len(h) >= epoch:
-                return False  # something was reduced already: strict / skip semantics of the general path
-        for h in plain:
-            h.append(None)
-        pending = self._launch(None, reset=True, plan=plan)
-        self._version += 1
+        if plan.bound or (plan.vote is not None and _world(self._group)[0] > 1):
+            pending = self._slab_or_create().reduce(*plan.ranges, reset=True, launches=plan.launches)
         slots = self._deferred_slots
-        for m, h in pairs:
+        for m, h in plan.bound:
             slots.append((h, len(h)))
             h.append(_Deferred(pending, m))
             m.count = 0
+        for m, h in plan.unbound:
+            h.append(None)
+            m.count = 0
+        if pending is not None and plan.vote is not None:
+            plan.vote[-1] = _Deferred(pending, _VoteOnly())
+            slots.append((plan.vote, len(plan.vote) - 1))
+        self._closed += (prefix,)
         if not self.deferred:
             self._materialize()
-        return True
 
     def reduce_live(self, prefix=None):
         """Cross-rank view of the running values of all (prefix-matching) reduced metrics, WITHOUT closing the epoch:
         the per-step metric exchange of BASELINE configs 2/3.  Returns a mapping {name: handle}; `handle.value()`
         brings the number to the host (one event sync) when it is actually needed.  The selection (cell ranges, layout
         hash) is cached while the metric set is unchanged, so the per-step host cost does not grow with #metrics."""
-        by_name, plan = self.live_selection(prefix)
-        if not by_name:
+        plan = self._plan(prefix)
+        if not plan.by_name:
             return {}
-        pending = self._launch(None, reset=False, plan=plan)
-        return _LiveView(pending, by_name)
+        pending = self._slab_or_create().reduce(*plan.ranges, reset=False, launches=plan.launches)
+        return _LiveView(pending, plan.by_name)
 
     def live_selection(self, prefix=None):
         """({name: metric}, (global ranges, local ranges, layout hash)) of the running metrics a live exchange covers:
         every reduced metric that owns cells and has no value for this epoch yet.  Cached while the metric set is
         unchanged, so the per-step host cost does not grow with #metrics."""
-        key = (self._version, prefix, self.epoch)
-        if self._live_plan is None or self._live_plan[0] != key:
-            # right after an epoch boundary nothing has a value yet: the selection is "every bound reduced metric", which
-            # only changes with the metric set (`_layout_version`), not with the epoch — no O(#metrics) planning per epoch
-            full = self._live_full.get(prefix)
-            fresh = full is not None and full[0] == self._layout_version and not self._reduced_this_epoch
-            if fresh:
-                self._live_plan = (key, full[1], full[2])
-            else:
-                metrics = [m for name, m in self.reducers.items()
-                           if (prefix is None or name.startswith(prefix)) and m.cell is not None
-                           and not self.has_value(name)]
-                self._live_plan = (key, {m.name: m for m in metrics}, self._plan(metrics) if metrics else None)
-                if not self._reduced_this_epoch:
-                    if len(self._live_full) > 16:
-                        self._live_full.clear()
-                    self._live_full[prefix] = (self._layout_version, self._live_plan[1], self._live_plan[2])
-        return self._live_plan[1], self._live_plan[2]
+        plan = self._plan(prefix)
+        return plan.by_name, plan.ranges
 
     def live_view(self, pending, by_name):
         """Mapping name -> handle over an exchange somebody else launched (the fused step exchange of a captured step)."""
@@ -1275,7 +1191,7 @@ class MetricTracker:
         """Reduces all metrics (if not already reduced) and advances the epoch counter (reference 275-280)."""
         self.reduce_all(strict=False)
         self.epoch += 1
-        self._reduced_this_epoch = False
+        self._closed = ()
 
     # -- checkpoint (reference 282-296) ------------------------------------------------------------------------------
     def state_dict(self, device_tensors=False):
@@ -1289,13 +1205,7 @@ class MetricTracker:
 
     def load_state_dict(self, state):
         self.epoch = state['epoch']
-        self._histories = {name: list(history) for name, history in state['histories'].items()}
-        self._deferred_slots = []
-        self._version += 1
-        self._layout_version += 1
-        self._reduce_cache = {}
-        self._live_full = {}
-        self._live_plan = None
+        self.histories = {name: list(history) for name, history in state['histories'].items()}
         self.reducers = {}
         for name, reducer_state in state['reducers'].items():
             metric = SlabMetric(self, name)

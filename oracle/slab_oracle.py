@@ -177,7 +177,7 @@ class OracleSlab:
             out = float(out)
         return out, (1 if empty == world else 0), status
 
-    def reduce(self, global_ranges, local_ranges, layout_hash, reset=True, exchange=True, to_host=True, plan_key=None):
+    def reduce(self, global_ranges, local_ranges, layout_hash, reset=True, exchange=True, to_host=True, launches=None):
         world, rank = _world(self.group)
         if not exchange:
             world = 1

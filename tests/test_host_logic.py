@@ -655,20 +655,29 @@ class TestPipelineHost:
         assert ran == [('b', 2), ('b', 3)]      # stage a is not run again; stage b continues at its 2nd epoch
         assert resumed.tracker.epoch == 6 and [v.item() for v in resumed.tracker['a/x'] if v is not None] == [1.0, 2.0]
 
-    def test_live_selection_is_planned_once_per_metric_set_not_once_per_epoch(self):
+    def test_live_selection_is_planned_once_per_metric_set_not_once_per_epoch(self, monkeypatch):
         """VERDICT r1 item 8: the 0.8 ms p99 of the per-step exchange was the live selection + layout hash of all 1024
         metrics being rebuilt after every next_epoch().  The plan object must survive epoch boundaries and change only
-        when the metric set does (or when part of the epoch has already been reduced)."""
+        when the metric set does (or when part of the epoch has already been reduced).  An epoch end right after a plain
+        metric was tracked (what Stage does with misc/epoch) reuses the plan too: no ranges or hash are rebuilt."""
+        from dmlcloud_b200 import metrics
         from dmlcloud_b200.metrics import MetricTracker, Reduction
 
+        hashed = []
+        layout_hash = metrics._layout_hash
+        monkeypatch.setattr(metrics, '_layout_hash', lambda items: hashed.append(len(items)) or layout_hash(items))
         t = MetricTracker()
         t.bind(slab=OracleSlab())
+        t.register_metric('misc/epoch')
         for i in range(64):
             t.register_metric(f'm{i}', Reduction.MEAN)
             t.track(f'm{i}', float(i))
         names, plan = t.live_selection()
         assert len(names) == 64
+        planned = len(hashed)
+        t.track('misc/epoch', 1)
         t.next_epoch()
+        assert len(hashed) == planned and t['misc/epoch'] == [1] and t['m5'][0].item() == 5.0
         for i in range(64):
             t.track(f'm{i}', 1.0)
         names2, plan2 = t.live_selection()
@@ -683,6 +692,87 @@ class TestPipelineHost:
             t.track(f'm{i}', 1.0)
         names4, plan4 = t.live_selection()
         assert 'late' in names4 and len(names4) == 65 and plan4 is not plan
+
+    def test_assigned_histories_are_the_ones_that_grow(self):
+        """Assigning `tracker.histories` replaces the lists later reduces append to, including the cached plans' ones."""
+        from dmlcloud_b200.metrics import Reduction
+
+        t = make_tracker()
+        t.register_metric('x', Reduction.SUM)
+        t.track('x', 1.0)
+        t.next_epoch()
+        t.histories = {name: list(history) for name, history in t.histories.items()}
+        t.track('x', 2.0)
+        t.next_epoch()
+        assert [v.item() for v in t['x']] == [1.0, 2.0]
+
+        # histories restored with a value for the current epoch already in them: only that epoch skips the metric
+        src = make_tracker()
+        for name in ('a', 'b'):
+            src.register_metric(name, Reduction.SUM)
+        src.track('a', 1.0)
+        src.track('b', 2.0)
+        src.reduce_all(prefix='a')
+        t = make_tracker()
+        t.load_state_dict(src.state_dict())
+        assert list(t.live_selection()[0]) == ['b']
+        t.next_epoch()
+        t.track('a', 3.0)
+        t.track('b', 4.0)
+        assert list(t.live_selection()[0]) == ['a', 'b']
+        t.next_epoch()
+        assert [v.item() for v in t['a']] == [1.0, 3.0] and [v.item() for v in t['b']] == [2.0, 4.0]
+
+    def test_plans_of_epochs_that_close_different_prefixes(self):
+        """Plans are cached per (prefix, metric set, prefixes closed this epoch).  Sessions that close different
+        prefixes in different epochs, register metrics after a closure and repeat a non-strict reduce see the same live
+        selections and histories as a tracker that plans every call afresh."""
+        from dmlcloud_b200.metrics import Reduction, _Plan
+
+        def session(t):
+            seen = []
+            for name in ('a/x', 'b/y', 'c/z'):
+                t.register_metric(name, Reduction.SUM)
+            t.register_metric('plain')
+            for epoch, (closes, late) in enumerate([('a', None), ('b', None), ('a', 'a/late'), ('a', None), ('b', 'b/late')]):
+                for name in t.reducers:
+                    if name != late:
+                        t.track(name, float(10 * epoch + len(name)))
+                t.track('plain', epoch)
+                t.reduce_all(prefix=closes)
+                seen.append(list(t.live_selection()[0]))
+                if late is not None:
+                    t.register_metric(late, Reduction.MAX)
+                    t.track(late, float(epoch))
+                    seen.append(list(t.live_selection()[0]))
+                t.reduce_all(prefix=closes, strict=False)
+                seen.append(list(t.live_selection('a')[0]))
+                t.next_epoch()
+            return seen, {name: [v.item() if isinstance(v, torch.Tensor) else v for v in h]
+                          for name, h in t.histories.items()}
+
+        uncached = make_tracker()
+        uncached._plan = lambda prefix: _Plan(uncached, prefix)
+        want = session(uncached)
+        assert want[0][:3] == [['b/y', 'c/z'], [], ['a/x', 'c/z']]
+        assert session(make_tracker()) == want
+
+    def test_strict_reduce_of_a_partly_closed_prefix_appends_nothing(self):
+        from dmlcloud_b200.metrics import Reduction
+
+        t = make_tracker()
+        t.register_metric('a/p')
+        t.register_metric('a/x', Reduction.SUM)
+        t.register_metric('a/y', Reduction.SUM)
+        t.track('a/x', 1.0)
+        t.track('a/y', 2.0)
+        t.reduce_all(prefix='a/x')
+        launches = list(t._slab.launches)
+        with pytest.raises(ValueError, match='History for a/x has already been reduced for epoch 1'):
+            t.reduce_all(prefix='a')
+        assert t._slab.launches == launches and t._histories['a/p'] == [] and t._histories['a/y'] == []
+        t.reduce_all(prefix='a', strict=False)
+        assert t.current_value('a/y').item() == 2.0 and t.current_value('a/p') is None
 
 
 # ------------------------------------------------------------------------------------------------------ W = 2 over gloo
