@@ -40,43 +40,133 @@ constexpr size_t kTmaMinElems = 32u << 20;
 constexpr int kUnroll = 4;      // independent vector loads a thread issues before its first store
 constexpr int kCtasPerSm = 4;
 
-// Each functor says how many elements one of its vector items covers (4: one 128-bit fp32 access; 8: one 128-bit bf16
-// access).
-template <class F>
-struct elems_of {
-    static constexpr int value = 4;
-};
-// ... and how many items a thread keeps in flight (register budget: 32 regs/thread for 4 CTAs x 512 threads per SM)
-template <class F>
-struct unroll_of {
-    static constexpr int value = kUnroll;
+// ---- functors: In = what one vector load returns, ld/st on vector index, scalar fallbacks on element index ---------
+// Each one says how many elements one of its vector items covers (kElems) and runs its own per-thread prologue.
+
+// A bucket's element type: its 128-bit access (kElems elements), the read-once load of it, the scalar fallback (widened to
+// fp32, stored back RNE) and the arithmetic on a whole access.
+template <class T>
+struct Elem;
+
+template <>
+struct Elem<float> {
+    typedef float4 V;
+    static constexpr int kElems = 4;
+    __device__ static __forceinline__ V ld_stream(const V *p) { return ld_stream_f4(p); }
+    __device__ static __forceinline__ float get(const float *p, size_t e) { return p[e]; }
+    __device__ static __forceinline__ void put(float *p, size_t e, float v) { p[e] = v; }
+    __device__ static __forceinline__ V scale(V v, float s) {
+        v.x *= s, v.y *= s, v.z *= s, v.w *= s;
+        return v;
+    }
+    __device__ static __forceinline__ double sumsq(V v) {
+        return (double)v.x * v.x + (double)v.y * v.y + (double)v.z * v.z + (double)v.w * v.w;
+    }
 };
 
-// ---- functors: In = what one vector load returns, ld/st on vector index, scalar fallbacks on element index ---------
-struct ScaleInplace {  // buf *= s                                   8 B/elem
-    typedef float4 In;
-    float *base;      // original pointer (scalar head/tail)
-    float4 *vec;      // aligned body
+// bf16 (DDP's bucket of bf16 parameters): one 128-bit access = 8 elements, arithmetic in fp32, stores RNE
+__device__ __forceinline__ uint32_t scale_bf16x2(uint32_t w, float s) { return pack_bf16x2(bf16_lo(w) * s, bf16_hi(w) * s); }
+__device__ __forceinline__ double sumsq_bf16x2(uint32_t w) {
+    const double lo = bf16_lo(w), hi = bf16_hi(w);
+    return lo * lo + hi * hi;
+}
+
+template <>
+struct Elem<uint16_t> {
+    typedef uint4 V;
+    static constexpr int kElems = 8;
+    __device__ static __forceinline__ V ld_stream(const V *p) { return ld_stream_u4(p); }
+    __device__ static __forceinline__ float get(const uint16_t *p, size_t e) { return bf16_to_f32(p[e]); }
+    __device__ static __forceinline__ void put(uint16_t *p, size_t e, float v) { p[e] = f32_to_bf16(v); }
+    __device__ static __forceinline__ V scale(V v, float s) {
+        v.x = scale_bf16x2(v.x, s), v.y = scale_bf16x2(v.y, s), v.z = scale_bf16x2(v.z, s), v.w = scale_bf16x2(v.w, s);
+        return v;
+    }
+    __device__ static __forceinline__ double sumsq(V v) {
+        return sumsq_bf16x2(v.x) + sumsq_bf16x2(v.y) + sumsq_bf16x2(v.z) + sumsq_bf16x2(v.w);
+    }
+};
+
+template <class T>
+struct Scale {  // buf = T(float(buf) * s)                 fp32: 8 B/elem; bf16: 4 B/elem, the NCCL route's K1 for a bf16 bucket
+    typedef Elem<T> E;
+    typedef typename E::V In;
+    static constexpr int kElems = E::kElems;
+    T *base;  // original pointer (scalar head/tail)
+    In *vec;  // aligned body
     float s;
+    __device__ __forceinline__ void prologue() {}
     __device__ __forceinline__ In ld(size_t i) const { return vec[i]; }  // read-write buffer: coherent path
     __device__ __forceinline__ double st(size_t i, In v) const {
-        v.x *= s, v.y *= s, v.z *= s, v.w *= s;
-        vec[i] = v;
+        vec[i] = E::scale(v, s);
         return 0.0;
     }
     __device__ __forceinline__ double scalar(size_t e) const {
-        base[e] *= s;
+        E::put(base, e, E::get(base, e) * s);
         return 0.0;
     }
 };
 
+template <class T>
+struct Sumsq {  // sum float(buf)^2                        fp32: 4 B/elem; bf16: 2 B/elem
+    typedef Elem<T> E;
+    typedef typename E::V In;
+    static constexpr int kElems = E::kElems;
+    const T *src;
+    const In *vsrc;
+    __device__ __forceinline__ void prologue() {}
+    __device__ __forceinline__ In ld(size_t i) const { return E::ld_stream(vsrc + i); }
+    __device__ __forceinline__ double st(size_t, In v) const { return E::sumsq(v); }
+    __device__ __forceinline__ double scalar(size_t e) const {
+        const double f = E::get(src, e);
+        return f * f;
+    }
+};
+
+template <class T>
+struct Clip {  // buf = T(float(buf) * min(1, max_norm / (sqrt(*sumsq) + 1e-6)))   fp32: 8 B/elem; bf16: 4 B/elem
+    typedef Elem<T> E;
+    typedef typename E::V In;
+    static constexpr int kElems = E::kElems;
+    T *base;
+    In *vec;
+    const double *sumsq;
+    float max_norm;
+    float coef;  // read on the device, per thread, by the prologue
+    // torch.nn.utils.clip_grad_norm_: clip_coef = max_norm / (total_norm + 1e-6), clamped to 1.0, all in fp32
+    __device__ __forceinline__ void prologue() {
+        float total = (float)sqrt(*sumsq);
+        float c = max_norm / (total + 1e-6f);
+        coef = c > 1.0f ? 1.0f : c;
+    }
+    __device__ __forceinline__ In ld(size_t i) const { return vec[i]; }
+    __device__ __forceinline__ double st(size_t i, In v) const {
+        vec[i] = E::scale(v, coef);
+        return 0.0;
+    }
+    __device__ __forceinline__ double scalar(size_t e) const {
+        E::put(base, e, E::get(base, e) * coef);
+        return 0.0;
+    }
+};
+
+// The instances launched, under the kernel names that launch traces and profiles identify them by
+struct ScaleInplace : Scale<float> {};
+struct ScaleBf16Inplace : Scale<uint16_t> {};
+struct SumsqF32 : Sumsq<float> {};
+struct SumsqBf16 : Sumsq<uint16_t> {};
+struct ClipF32 : Clip<float> {};
+struct ClipBf16 : Clip<uint16_t> {};
+
 struct PackF32 {  // dst = src * s                                   8 B/elem
     typedef float4 In;
+    static constexpr int kElems = 4;
     const float *src;
     float *dst;
     const float4 *vsrc;
     float4 *vdst;
     float s;
+    __device__ __forceinline__ void prologue() {}
     __device__ __forceinline__ In ld(size_t i) const { return ld_stream_f4(vsrc + i); }
     __device__ __forceinline__ double st(size_t i, In v) const {
         v.x *= s, v.y *= s, v.z *= s, v.w *= s;
@@ -91,11 +181,13 @@ struct PackF32 {  // dst = src * s                                   8 B/elem
 
 struct PackBf16 {  // dst = bf16_rn(src * s)                         6 B/elem
     typedef float4 In;
+    static constexpr int kElems = 4;
     const float *src;
     uint16_t *dst;
     const float4 *vsrc;
     uint2 *vdst;
     float s;
+    __device__ __forceinline__ void prologue() {}
     __device__ __forceinline__ In ld(size_t i) const { return ld_stream_f4(vsrc + i); }
     __device__ __forceinline__ double st(size_t i, In v) const {
         uint2 o;
@@ -113,11 +205,13 @@ struct PackBf16 {  // dst = bf16_rn(src * s)                         6 B/elem
 template <bool kSumsq>
 struct UnpackBf16 {  // dst = float(src) * s  (+ sum dst^2)          6 B/elem
     typedef uint2 In;
+    static constexpr int kElems = 4;
     const uint16_t *src;
     float *dst;
     const uint2 *vsrc;
     float4 *vdst;
     float s;
+    __device__ __forceinline__ void prologue() {}
     __device__ __forceinline__ In ld(size_t i) const { return ld_stream_u2(vsrc + i); }
     __device__ __forceinline__ double st(size_t i, In v) const {
         float4 o;
@@ -136,10 +230,12 @@ struct UnpackBf16 {  // dst = float(src) * s  (+ sum dst^2)          6 B/elem
 template <bool kSumsq>
 struct RoundBf16Inplace {  // buf = float(bf16_rn(buf * s))  (+ sum buf^2)   8 B/elem — the W == 1 form of the bf16 wire
     typedef float4 In;
+    static constexpr int kElems = 4;
     float *base;
     float4 *vec;
     float s;
     __device__ __forceinline__ static float rt(float f) { return bf16_to_f32(f32_to_bf16(f)); }
+    __device__ __forceinline__ void prologue() {}
     __device__ __forceinline__ In ld(size_t i) const { return vec[i]; }
     __device__ __forceinline__ double st(size_t i, In v) const {
         v.x = rt(v.x * s), v.y = rt(v.y * s), v.z = rt(v.z * s), v.w = rt(v.w * s);
@@ -154,128 +250,14 @@ struct RoundBf16Inplace {  // buf = float(bf16_rn(buf * s))  (+ sum buf^2)   8 B
     }
 };
 
-struct SumsqF32 {  // sum buf^2                                      4 B/elem
-    typedef float4 In;
-    const float *src;
-    const float4 *vsrc;
-    __device__ __forceinline__ In ld(size_t i) const { return ld_stream_f4(vsrc + i); }
-    __device__ __forceinline__ double st(size_t, In v) const {
-        return (double)v.x * v.x + (double)v.y * v.y + (double)v.z * v.z + (double)v.w * v.w;
-    }
-    __device__ __forceinline__ double scalar(size_t e) const { return (double)src[e] * src[e]; }
-};
-
-struct ClipF32 {  // buf *= min(1, max_norm / (sqrt(*sumsq) + 1e-6))   8 B/elem, coefficient read on device
-    typedef float4 In;
-    float *base;
-    float4 *vec;
-    const double *sumsq;
-    float max_norm;
-    float coef;  // filled per thread in the kernel prologue
-    __device__ __forceinline__ In ld(size_t i) const { return vec[i]; }
-    __device__ __forceinline__ double st(size_t i, In v) const {
-        v.x *= coef, v.y *= coef, v.z *= coef, v.w *= coef;
-        vec[i] = v;
-        return 0.0;
-    }
-    __device__ __forceinline__ double scalar(size_t e) const {
-        base[e] *= coef;
-        return 0.0;
-    }
-};
-
-// ---- bf16 buckets (DDP's bucket of bf16 parameters): one 128-bit access = 8 elements, arithmetic in fp32, stores RNE --
-__device__ __forceinline__ uint32_t scale_bf16x2(uint32_t w, float s) { return pack_bf16x2(bf16_lo(w) * s, bf16_hi(w) * s); }
-__device__ __forceinline__ uint4 scale_bf16x8(uint4 v, float s) {
-    v.x = scale_bf16x2(v.x, s), v.y = scale_bf16x2(v.y, s), v.z = scale_bf16x2(v.z, s), v.w = scale_bf16x2(v.w, s);
-    return v;
-}
-__device__ __forceinline__ double sumsq_bf16x2(uint32_t w) {
-    const double lo = bf16_lo(w), hi = bf16_hi(w);
-    return lo * lo + hi * hi;
-}
-
-struct ScaleBf16Inplace {  // buf = bf16_rn(float(buf) * s)            4 B/elem — the NCCL route's K1 for a bf16 bucket
-    typedef uint4 In;
-    uint16_t *base;
-    uint4 *vec;
-    float s;
-    __device__ __forceinline__ In ld(size_t i) const { return vec[i]; }
-    __device__ __forceinline__ double st(size_t i, In v) const {
-        vec[i] = scale_bf16x8(v, s);
-        return 0.0;
-    }
-    __device__ __forceinline__ double scalar(size_t e) const {
-        base[e] = f32_to_bf16(bf16_to_f32(base[e]) * s);
-        return 0.0;
-    }
-};
-
-struct SumsqBf16 {  // sum float(buf)^2                              2 B/elem
-    typedef uint4 In;
-    const uint16_t *src;
-    const uint4 *vsrc;
-    __device__ __forceinline__ In ld(size_t i) const { return ld_stream_u4(vsrc + i); }
-    __device__ __forceinline__ double st(size_t, In v) const {
-        return sumsq_bf16x2(v.x) + sumsq_bf16x2(v.y) + sumsq_bf16x2(v.z) + sumsq_bf16x2(v.w);
-    }
-    __device__ __forceinline__ double scalar(size_t e) const {
-        const double f = bf16_to_f32(src[e]);
-        return f * f;
-    }
-};
-
-struct ClipBf16 {  // buf = bf16_rn(float(buf) * coef), coef as ClipF32's  4 B/elem
-    typedef uint4 In;
-    uint16_t *base;
-    uint4 *vec;
-    const double *sumsq;
-    float max_norm;
-    float coef;  // filled per thread in the kernel prologue
-    __device__ __forceinline__ In ld(size_t i) const { return vec[i]; }
-    __device__ __forceinline__ double st(size_t i, In v) const {
-        vec[i] = scale_bf16x8(v, coef);
-        return 0.0;
-    }
-    __device__ __forceinline__ double scalar(size_t e) const {
-        base[e] = f32_to_bf16(bf16_to_f32(base[e]) * coef);
-        return 0.0;
-    }
-};
-
-template <>
-struct elems_of<ScaleBf16Inplace> {
-    static constexpr int value = 8;
-};
-template <>
-struct elems_of<SumsqBf16> {
-    static constexpr int value = 8;
-};
-template <>
-struct elems_of<ClipBf16> {
-    static constexpr int value = 8;
-};
-
-// torch.nn.utils.clip_grad_norm_: clip_coef = max_norm / (total_norm + 1e-6), clamped to 1.0, all in fp32
-template <class F>
-__device__ __forceinline__ void clip_prologue(F &f) {
-    float total = (float)sqrt(*f.sumsq);
-    float c = f.max_norm / (total + 1e-6f);
-    f.coef = c > 1.0f ? 1.0f : c;
-}
-__device__ __forceinline__ void prologue(ClipF32 &f) { clip_prologue(f); }
-__device__ __forceinline__ void prologue(ClipBf16 &f) { clip_prologue(f); }
-template <class F>
-__device__ __forceinline__ void prologue(F &) {}
-
-// One streaming kernel for all of the above.  head = scalar elements before the aligned body, nvec = 4-element vectors
+// One streaming kernel for all of the above.  head = scalar elements before the aligned body, nvec = vector items
 // in the body, n = total elements.
 template <class F, bool kReduce>
 __global__ void __launch_bounds__(kThreads, kCtasPerSm)
 stream_kernel(F f, size_t head, size_t nvec, size_t n, double *sumsq_out, size_t chunk) {
-    prologue(f);
+    f.prologue();
     double part = 0.0;
-    constexpr int U = unroll_of<F>::value;
+    constexpr int U = kUnroll;
     // chunk == 0: grid-stride sweeps (large inputs: the whole grid walks one ~17 MB window at a time).
     // chunk  > 0: CTA b owns vectors [b * chunk, (b + 1) * chunk) — DDP-bucket-sized inputs are one or two waves long, and
     //             with work handed out in fixed 2048-vector blocks some SMs get 4 CTAs' worth and others 3 (a 3.96 M
@@ -302,7 +284,7 @@ stream_kernel(F f, size_t head, size_t nvec, size_t n, double *sumsq_out, size_t
         if (t < 8) {
             if (t < head) part += f.scalar(t);
         } else {
-            size_t e = head + nvec * elems_of<F>::value + (t - 8);
+            size_t e = head + nvec * F::kElems + (t - 8);
             if (e < n) part += f.scalar(e);
         }
     }
@@ -315,7 +297,7 @@ stream_kernel(F f, size_t head, size_t nvec, size_t n, double *sumsq_out, size_t
 // scalar fallback when the two pointers cannot be brought to vector alignment together
 template <class F, bool kReduce>
 __global__ void __launch_bounds__(kThreads) scalar_kernel(F f, size_t n, double *sumsq_out) {
-    prologue(f);
+    f.prologue();
     double part = 0.0;
     for (size_t e = (size_t)blockIdx.x * kThreads + threadIdx.x; e < n; e += (size_t)gridDim.x * kThreads)
         part += f.scalar(e);
@@ -334,17 +316,36 @@ static inline long head_for(const void *p, size_t esz, size_t align) {
     return (long)(need / esz);
 }
 
-template <class F, bool kReduce>
-static int launch_stream(F f, long head, size_t n, double *sumsq, cudaStream_t st) {
+// The entry points' view of their operands, src and dst (the same buffer for an in-place kernel): EINVAL for a missing
+// operand, EALIGN for one not aligned to its element, else `head`, the elements before a body of E-element vector items
+// aligned in both (-1 when there is none: the scalar kernel takes the buffer).
+template <int E, class S, class D>
+static int split(const S *src, const D *dst, size_t n, long &head) {
+    if ((!src || !dst) && n) return DMLB_EINVAL;
+    if (((uintptr_t)src % sizeof(S)) || ((uintptr_t)dst % sizeof(D))) return DMLB_EALIGN;
+    head = head_for(src, sizeof(S), E * sizeof(S));
+    if (head >= 0 && ((uintptr_t)(dst + head) % (E * sizeof(D)))) head = -1;
+    return DMLB_OK;
+}
+
+// the vector body of p: what follows its `head` elements
+template <class V, class T>
+static V *body(T *p, long head) {
+    return reinterpret_cast<V *>(p + (head > 0 ? head : 0));
+}
+
+template <bool kReduce, class F>
+static int launch_stream(F f, long head, size_t n, double *sumsq, void *stream) {
     if (n == 0) return DMLB_OK;
+    const cudaStream_t st = (cudaStream_t)stream;
     if (head < 0) {
         int grid = stream_grid(n, 1, kCtasPerSm);
         scalar_kernel<F, kReduce><<<grid, kThreads, 0, st>>>(f, n, sumsq);
         return launched();
     }
     size_t h = (size_t)head < n ? (size_t)head : n;
-    size_t nvec = (n - h) / elems_of<F>::value;
-    const size_t per_cta = (size_t)kThreads * unroll_of<F>::value;
+    size_t nvec = (n - h) / F::kElems;
+    const size_t per_cta = (size_t)kThreads * kUnroll;
     const size_t want = (nvec + per_cta - 1) / per_cta;
     const size_t sms = (size_t)sm_count(), cap = sms * kCtasPerSm;
     int grid;
@@ -356,10 +357,34 @@ static int launch_stream(F f, long head, size_t n, double *sumsq, cudaStream_t s
         chunk = (nvec + g - 1) / g;
         if (chunk < 1) chunk = 1;
     } else {
-        grid = stream_grid(nvec, unroll_of<F>::value, kCtasPerSm);
+        grid = stream_grid(nvec, kUnroll, kCtasPerSm);
     }
     stream_kernel<F, kReduce><<<grid, kThreads, 0, st>>>(f, h, nvec, n, sumsq, chunk);
     return launched();
+}
+
+// F: one of the named Scale / Sumsq / Clip instances below, T: its element type
+template <class F, class T>
+static int scale_inplace(T *buf, size_t n, float scale, void *stream) {
+    long head;
+    if (int rc = split<F::kElems>(buf, buf, n, head)) return rc;
+    return launch_stream<false>(F{{buf, body<typename F::In>(buf, head), scale}}, head, n, nullptr, stream);
+}
+
+template <class F, class T>
+static int sumsq_of(const T *buf, size_t n, double *sumsq, void *stream) {
+    long head;
+    if (!sumsq) return DMLB_EINVAL;
+    if (int rc = split<F::kElems>(buf, buf, n, head)) return rc;
+    return launch_stream<true>(F{{buf, body<const typename F::In>(buf, head)}}, head, n, sumsq, stream);
+}
+
+template <class F, class T>
+static int clip(T *buf, size_t n, const double *sumsq, float max_norm, void *stream) {
+    long head;
+    if (!sumsq) return DMLB_EINVAL;
+    if (int rc = split<F::kElems>(buf, buf, n, head)) return rc;
+    return launch_stream<false>(F{{buf, body<typename F::In>(buf, head), sumsq, max_norm, 1.0f}}, head, n, nullptr, stream);
 }
 
 }  // namespace dmlb
@@ -369,50 +394,34 @@ using namespace dmlb;
 extern "C" {
 
 int dmlb_bucket_scale_f32(float *buf, size_t n, float scale, void *stream) {
-    if (!buf && n) return DMLB_EINVAL;
-    if ((uintptr_t)buf & 3) return DMLB_EALIGN;
-    long head = head_for(buf, 4, 16);
-    ScaleInplace f{buf, reinterpret_cast<float4 *>(buf + (head > 0 ? head : 0)), scale};
-    return launch_stream<ScaleInplace, false>(f, head, n, nullptr, (cudaStream_t)stream);
+    return scale_inplace<ScaleInplace>(buf, n, scale, stream);
 }
 
 int dmlb_bucket_pack_f32_f32(const float *src, float *dst, size_t n, float scale, void *stream) {
-    if ((!src || !dst) && n) return DMLB_EINVAL;
-    if (((uintptr_t)src & 3) || ((uintptr_t)dst & 3)) return DMLB_EALIGN;
-    long head = head_for(src, 4, 16);
-    if (head >= 0 && (((uintptr_t)(dst + head)) & 15)) head = -1;
-    size_t h = head > 0 ? head : 0;
-    PackF32 f{src, dst, reinterpret_cast<const float4 *>(src + h), reinterpret_cast<float4 *>(dst + h), scale};
-    return launch_stream<PackF32, false>(f, head, n, nullptr, (cudaStream_t)stream);
+    long head;
+    if (int rc = split<4>(src, dst, n, head)) return rc;
+    PackF32 f{src, dst, body<const float4>(src, head), body<float4>(dst, head), scale};
+    return launch_stream<false>(f, head, n, nullptr, stream);
 }
 
-static int pack_bf16_regs(const float *src, uint16_t *dst, size_t n, float scale, void *stream);
-
 int dmlb_bucket_pack_f32_bf16_regs(const float *src, uint16_t *dst, size_t n, float scale, void *stream) {
-    if ((!src || !dst) && n) return DMLB_EINVAL;
-    if (((uintptr_t)src & 3) || ((uintptr_t)dst & 1)) return DMLB_EALIGN;
-    return pack_bf16_regs(src, dst, n, scale, stream);
+    long head;
+    if (int rc = split<4>(src, dst, n, head)) return rc;
+    PackBf16 f{src, dst, body<const float4>(src, head), body<uint2>(dst, head), scale};
+    return launch_stream<false>(f, head, n, nullptr, stream);
 }
 
 int dmlb_bucket_pack_f32_bf16(const float *src, uint16_t *dst, size_t n, float scale, void *stream) {
-    if ((!src || !dst) && n) return DMLB_EINVAL;
-    if (((uintptr_t)src & 3) || ((uintptr_t)dst & 1)) return DMLB_EALIGN;
+    long head;
+    if (int rc = split<4>(src, dst, n, head)) return rc;
     if (n >= kTmaMinElems && (((uintptr_t)src) & 15) == 0 && (((uintptr_t)dst) & 15) == 0)
         return dmlb_bucket_pack_f32_bf16_tma(src, dst, n, scale, stream);  // huge + aligned: TMA bulk loads (0.96 vs 0.93)
-    return pack_bf16_regs(src, dst, n, scale, stream);
-}
-
-static int pack_bf16_regs(const float *src, uint16_t *dst, size_t n, float scale, void *stream) {
-    long head = head_for(src, 4, 16);
-    if (head >= 0 && (((uintptr_t)(dst + head)) & 7)) head = -1;
-    size_t h = head > 0 ? head : 0;
-    PackBf16 f{src, dst, reinterpret_cast<const float4 *>(src + h), reinterpret_cast<uint2 *>(dst + h), scale};
-    return launch_stream<PackBf16, false>(f, head, n, nullptr, (cudaStream_t)stream);
+    return dmlb_bucket_pack_f32_bf16_regs(src, dst, n, scale, stream);
 }
 
 int dmlb_bucket_unpack_bf16_f32(const uint16_t *src, float *dst, size_t n, float scale, double *sumsq, void *stream) {
-    if ((!src || !dst) && n) return DMLB_EINVAL;
-    if (((uintptr_t)src & 1) || ((uintptr_t)dst & 3)) return DMLB_EALIGN;
+    long head;
+    if (int rc = split<4>(src, dst, n, head)) return rc;
     if (!sumsq && n >= kTmaMinElems && (((uintptr_t)src) & 15) == 0 && (((uintptr_t)dst) & 15) == 0)
         return dmlb_bucket_unpack_bf16_f32_tma(src, dst, n, scale, stream);  // TMA bulk load + bulk store
     return dmlb_bucket_unpack_bf16_f32_regs(src, dst, n, scale, sumsq, stream);
@@ -420,71 +429,40 @@ int dmlb_bucket_unpack_bf16_f32(const uint16_t *src, float *dst, size_t n, float
 
 int dmlb_bucket_unpack_bf16_f32_regs(const uint16_t *src, float *dst, size_t n, float scale, double *sumsq,
                                      void *stream) {
-    if ((!src || !dst) && n) return DMLB_EINVAL;
-    if (((uintptr_t)src & 1) || ((uintptr_t)dst & 3)) return DMLB_EALIGN;
-    long head = head_for(dst, 4, 16);
-    if (head >= 0 && (((uintptr_t)(src + head)) & 7)) head = -1;
-    size_t h = head > 0 ? head : 0;
-    if (sumsq) {
-        UnpackBf16<true> f{src, dst, reinterpret_cast<const uint2 *>(src + h), reinterpret_cast<float4 *>(dst + h),
-                           scale};
-        return launch_stream<UnpackBf16<true>, true>(f, head, n, sumsq, (cudaStream_t)stream);
-    }
-    UnpackBf16<false> f{src, dst, reinterpret_cast<const uint2 *>(src + h), reinterpret_cast<float4 *>(dst + h), scale};
-    return launch_stream<UnpackBf16<false>, false>(f, head, n, nullptr, (cudaStream_t)stream);
+    long head;
+    if (int rc = split<4>(src, dst, n, head)) return rc;
+    const uint2 *vsrc = body<const uint2>(src, head);
+    float4 *vdst = body<float4>(dst, head);
+    if (sumsq) return launch_stream<true>(UnpackBf16<true>{src, dst, vsrc, vdst, scale}, head, n, sumsq, stream);
+    return launch_stream<false>(UnpackBf16<false>{src, dst, vsrc, vdst, scale}, head, n, nullptr, stream);
 }
 
 int dmlb_bucket_round_bf16_f32(float *buf, size_t n, float scale, double *sumsq, void *stream) {
-    if (!buf && n) return DMLB_EINVAL;
-    if ((uintptr_t)buf & 3) return DMLB_EALIGN;
-    long head = head_for(buf, 4, 16);
-    float4 *vec = reinterpret_cast<float4 *>(buf + (head > 0 ? head : 0));
-    if (sumsq) {
-        RoundBf16Inplace<true> f{buf, vec, scale};
-        return launch_stream<RoundBf16Inplace<true>, true>(f, head, n, sumsq, (cudaStream_t)stream);
-    }
-    RoundBf16Inplace<false> f{buf, vec, scale};
-    return launch_stream<RoundBf16Inplace<false>, false>(f, head, n, nullptr, (cudaStream_t)stream);
+    long head;
+    if (int rc = split<4>(buf, buf, n, head)) return rc;
+    float4 *vec = body<float4>(buf, head);
+    if (sumsq) return launch_stream<true>(RoundBf16Inplace<true>{buf, vec, scale}, head, n, sumsq, stream);
+    return launch_stream<false>(RoundBf16Inplace<false>{buf, vec, scale}, head, n, nullptr, stream);
 }
 
 int dmlb_bucket_sumsq_f32(const float *buf, size_t n, double *sumsq, void *stream) {
-    if ((!buf && n) || !sumsq) return DMLB_EINVAL;
-    if ((uintptr_t)buf & 3) return DMLB_EALIGN;
-    long head = head_for(buf, 4, 16);
-    SumsqF32 f{buf, reinterpret_cast<const float4 *>(buf + (head > 0 ? head : 0))};
-    return launch_stream<SumsqF32, true>(f, head, n, sumsq, (cudaStream_t)stream);
+    return sumsq_of<SumsqF32>(buf, n, sumsq, stream);
 }
 
 int dmlb_bucket_clip_f32(float *buf, size_t n, const double *sumsq, float max_norm, void *stream) {
-    if ((!buf && n) || !sumsq) return DMLB_EINVAL;
-    if ((uintptr_t)buf & 3) return DMLB_EALIGN;
-    long head = head_for(buf, 4, 16);
-    ClipF32 f{buf, reinterpret_cast<float4 *>(buf + (head > 0 ? head : 0)), sumsq, max_norm, 1.0f};
-    return launch_stream<ClipF32, false>(f, head, n, nullptr, (cudaStream_t)stream);
+    return clip<ClipF32>(buf, n, sumsq, max_norm, stream);
 }
 
 int dmlb_bucket_scale_bf16(uint16_t *buf, size_t n, float scale, void *stream) {
-    if (!buf && n) return DMLB_EINVAL;
-    if ((uintptr_t)buf & 1) return DMLB_EALIGN;
-    long head = head_for(buf, 2, 16);
-    ScaleBf16Inplace f{buf, reinterpret_cast<uint4 *>(buf + head), scale};
-    return launch_stream<ScaleBf16Inplace, false>(f, head, n, nullptr, (cudaStream_t)stream);
+    return scale_inplace<ScaleBf16Inplace>(buf, n, scale, stream);
 }
 
 int dmlb_bucket_sumsq_bf16(const uint16_t *buf, size_t n, double *sumsq, void *stream) {
-    if ((!buf && n) || !sumsq) return DMLB_EINVAL;
-    if ((uintptr_t)buf & 1) return DMLB_EALIGN;
-    long head = head_for(buf, 2, 16);
-    SumsqBf16 f{buf, reinterpret_cast<const uint4 *>(buf + head)};
-    return launch_stream<SumsqBf16, true>(f, head, n, sumsq, (cudaStream_t)stream);
+    return sumsq_of<SumsqBf16>(buf, n, sumsq, stream);
 }
 
 int dmlb_bucket_clip_bf16(uint16_t *buf, size_t n, const double *sumsq, float max_norm, void *stream) {
-    if ((!buf && n) || !sumsq) return DMLB_EINVAL;
-    if ((uintptr_t)buf & 1) return DMLB_EALIGN;
-    long head = head_for(buf, 2, 16);
-    ClipBf16 f{buf, reinterpret_cast<uint4 *>(buf + head), sumsq, max_norm, 1.0f};
-    return launch_stream<ClipBf16, false>(f, head, n, nullptr, (cudaStream_t)stream);
+    return clip<ClipBf16>(buf, n, sumsq, max_norm, stream);
 }
 
 }  // extern "C"

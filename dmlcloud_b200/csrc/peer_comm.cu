@@ -36,12 +36,14 @@
 
 namespace dmlb {
 
+// The wire dtype: how a 16-byte wire vector packs from and accumulates into fp32, and the same for the 8-byte payload of an
+// LL line (the line's words x and z; ll_store puts the sequence number between them).
 template <int kWire>
 struct Wire;
 
 template <>
-struct Wire<DMLB_WIRE_F32> {  // 4 elements per 16-byte wire vector
-    static constexpr int kElems = 4;
+struct Wire<DMLB_WIRE_F32> {  // 4 elements per 16-byte wire vector, 2 per LL line
+    static constexpr int kElems = 4, kLineElems = 2;
     __device__ static __forceinline__ uint4 pack(const float *v) {
         uint4 o;
         o.x = __float_as_uint(v[0]), o.y = __float_as_uint(v[1]), o.z = __float_as_uint(v[2]), o.w = __float_as_uint(v[3]);
@@ -50,6 +52,10 @@ struct Wire<DMLB_WIRE_F32> {  // 4 elements per 16-byte wire vector
     __device__ static __forceinline__ void accumulate(float *acc, uint4 w) {
         acc[0] += __uint_as_float(w.x), acc[1] += __uint_as_float(w.y);
         acc[2] += __uint_as_float(w.z), acc[3] += __uint_as_float(w.w);
+    }
+    __device__ static __forceinline__ uint2 pack_line(const float *v) { return make_uint2(__float_as_uint(v[0]), __float_as_uint(v[1])); }
+    __device__ static __forceinline__ void accumulate_line(float *acc, uint4 w) {
+        acc[0] += __uint_as_float(w.x), acc[1] += __uint_as_float(w.z);
     }
     __device__ static __forceinline__ uint4 mc_reduce(const void *mc) {  // in-switch sum over all ranks' copies
         uint4 v;
@@ -62,8 +68,8 @@ struct Wire<DMLB_WIRE_F32> {  // 4 elements per 16-byte wire vector
 };
 
 template <>
-struct Wire<DMLB_WIRE_BF16> {  // 8 elements per 16-byte wire vector
-    static constexpr int kElems = 8;
+struct Wire<DMLB_WIRE_BF16> {  // 8 elements per 16-byte wire vector, 4 per LL line
+    static constexpr int kElems = 8, kLineElems = 4;
     __device__ static __forceinline__ uint4 pack(const float *v) {
         uint4 o;
         o.x = pack_bf16x2(v[0], v[1]), o.y = pack_bf16x2(v[2], v[3]);
@@ -73,6 +79,10 @@ struct Wire<DMLB_WIRE_BF16> {  // 8 elements per 16-byte wire vector
     __device__ static __forceinline__ void accumulate(float *acc, uint4 w) {
         acc[0] += bf16_lo(w.x), acc[1] += bf16_hi(w.x), acc[2] += bf16_lo(w.y), acc[3] += bf16_hi(w.y);
         acc[4] += bf16_lo(w.z), acc[5] += bf16_hi(w.z), acc[6] += bf16_lo(w.w), acc[7] += bf16_hi(w.w);
+    }
+    __device__ static __forceinline__ uint2 pack_line(const float *v) { return make_uint2(pack_bf16x2(v[0], v[1]), pack_bf16x2(v[2], v[3])); }
+    __device__ static __forceinline__ void accumulate_line(float *acc, uint4 w) {
+        acc[0] += bf16_lo(w.x), acc[1] += bf16_hi(w.x), acc[2] += bf16_lo(w.z), acc[3] += bf16_hi(w.z);
     }
     __device__ static __forceinline__ uint4 mc_reduce(const void *mc) {  // fp32 accumulation in the switch, bf16 result
         uint4 v;
@@ -146,9 +156,7 @@ __device__ __forceinline__ double store_bucket(T *bucket, size_t g, size_t n, co
         if constexpr (kBf16Bucket<T>) {
 #pragma unroll
             for (int j = 0; j < E; j += 8) {
-                uint4 o;
-                o.x = pack_bf16x2(v[j], v[j + 1]), o.y = pack_bf16x2(v[j + 2], v[j + 3]);
-                o.z = pack_bf16x2(v[j + 4], v[j + 5]), o.w = pack_bf16x2(v[j + 6], v[j + 7]);
+                const uint4 o = Wire<DMLB_WIRE_BF16>::pack(v + j);
                 *reinterpret_cast<uint4 *>(bucket + e0 + j) = o;
                 if (sumsq) {
                     const uint32_t w[4] = {o.x, o.y, o.z, o.w};
@@ -189,6 +197,18 @@ __device__ __forceinline__ double store_bucket(T *bucket, size_t g, size_t n, co
 template <int E, class T>
 __device__ __forceinline__ void poison_range(T *bucket, size_t lo, size_t hi, size_t n) {
     for (size_t e = lo * E + threadIdx.x; e < hi * E && e < n; e += kCommThreads) poison_elem(bucket, e);
+}
+
+// A CTA that poisoned its part of the bucket adds NaN to the fused sum of squares, so that clipping reports it too.
+__device__ __forceinline__ double poisoned_sumsq() { return __longlong_as_double(0x7ff8000000000000ll); }
+
+// The end of every data CTA: its part of the fused sum of squares, then the end of the collective.
+__device__ __forceinline__ void data_cta_end(const CommDev &c, uint32_t s, double part, double *sumsq_out) {
+    if (sumsq_out) {
+        double tot = block_sum(part);
+        if (threadIdx.x == 0 && tot != 0.0) atomicAdd(sumsq_out, tot);
+    }
+    comm_end(c, s);
 }
 
 // ---------------------------------------------------------------------------------------------------------------------
@@ -350,6 +370,15 @@ __device__ __noinline__ void metric_cta(const CommDev &c, uint32_t s, const dmlb
     }
 }
 
+// true for the metric CTA (the block after the n_data data CTAs) once it has run: the calling kernel returns
+template <bool kLL>
+__device__ __forceinline__ bool ran_metric_cta(const CommDev &c, uint32_t s, int n_data, const dmlb_step_metrics &M) {
+    if ((int)blockIdx.x < n_data) return false;
+    metric_cta<kLL>(c, s, M);
+    comm_end(c, s);
+    return true;
+}
+
 // ---------------------------------------------------------------------------------------------------------------------
 // one-shot
 // ---------------------------------------------------------------------------------------------------------------------
@@ -360,11 +389,7 @@ allreduce_oneshot_kernel(const __grid_constant__ CommDev c, T *bucket, size_t n,
     typedef Wire<kWire> W;
     constexpr int E = W::kElems;
     const uint32_t s = comm_begin(c);
-    if ((int)blockIdx.x >= n_data) {
-        metric_cta<false>(c, s, M);
-        comm_end(c, s);
-        return;
-    }
+    if (ran_metric_cta<false>(c, s, n_data, M)) return;
     const int half = s & 1;
     const size_t per = (nvec + n_data - 1) / n_data;
     const size_t lo = (size_t)blockIdx.x * per;
@@ -392,14 +417,10 @@ allreduce_oneshot_kernel(const __grid_constant__ CommDev c, T *bucket, size_t n,
             });
         } else {
             poison_range<E>(bucket, lo, hi, n);
-            part = __longlong_as_double(0x7ff8000000000000ll);
+            part = poisoned_sumsq();
         }
     }
-    if (sumsq_out) {
-        double tot = block_sum(part);
-        if (threadIdx.x == 0 && tot != 0.0) atomicAdd(sumsq_out, tot);
-    }
-    comm_end(c, s);
+    data_cta_end(c, s, part, sumsq_out);
 }
 
 // ---------------------------------------------------------------------------------------------------------------------
@@ -412,13 +433,10 @@ template <class T, int kWire>
 __global__ void __launch_bounds__(kCommThreads, 2)
 allreduce_ll_kernel(const __grid_constant__ CommDev c, T *bucket, size_t n, size_t n_lines, float scale,
                     double *sumsq_out, int n_data, const __grid_constant__ dmlb_step_metrics M) {
-    constexpr int EL = kWire == DMLB_WIRE_BF16 ? 4 : 2;  // elements per line
+    typedef Wire<kWire> W;
+    constexpr int EL = W::kLineElems;
     const uint32_t s = comm_begin(c);
-    if ((int)blockIdx.x >= n_data) {
-        metric_cta<true>(c, s, M);
-        comm_end(c, s);
-        return;
-    }
+    if (ran_metric_cta<true>(c, s, n_data, M)) return;
     const int half = s & 1;
     const size_t per = (n_lines + n_data - 1) / n_data;
     const size_t lo = (size_t)blockIdx.x * per;
@@ -429,17 +447,10 @@ allreduce_ll_kernel(const __grid_constant__ CommDev c, T *bucket, size_t n, size
         const size_t e0 = l * EL;
 #pragma unroll
         for (int j = 0; j < EL; ++j) v[j] = (e0 + j < n) ? ld_elem(bucket, e0 + j) * scale : 0.0f;
-        uint32_t d0, d1;
-        if (kWire == DMLB_WIRE_BF16) {
-            d0 = pack_bf16x2(v[0], v[1]);
-            d1 = pack_bf16x2(v[EL - 2], v[EL - 1]);
-        } else {
-            d0 = __float_as_uint(v[0]);
-            d1 = __float_as_uint(v[1]);
-        }
+        const uint2 d = W::pack_line(v);
 #pragma unroll
         for (int r = 0; r < DMLB_MAX_WORLD; ++r)
-            if (r < c.world) ll_store(c.ll(r, half, c.rank) + l, d0, d1, s);
+            if (r < c.world) ll_store(c.ll(r, half, c.rank) + l, d.x, d.y, s);
     }
     // pull + sum in rank order
     double part = 0.0;
@@ -454,14 +465,7 @@ allreduce_ll_kernel(const __grid_constant__ CommDev c, T *bucket, size_t n, size
         for (int j = 0; j < EL; ++j) acc[j] = -0.0f;
 #pragma unroll
         for (int r = 0; r < DMLB_MAX_WORLD; ++r)
-            if (r < c.world) {
-                if (kWire == DMLB_WIRE_BF16) {
-                    acc[0] += bf16_lo(w[r].x), acc[1] += bf16_hi(w[r].x);
-                    acc[EL - 2] += bf16_lo(w[r].z), acc[EL - 1] += bf16_hi(w[r].z);
-                } else {
-                    acc[0] += __uint_as_float(w[r].x), acc[1] += __uint_as_float(w[r].z);
-                }
-            }
+            if (r < c.world) W::accumulate_line(acc, w[r]);
         const size_t e0 = l * EL;
 #pragma unroll
         for (int j = 0; j < EL; ++j)
@@ -471,14 +475,10 @@ allreduce_ll_kernel(const __grid_constant__ CommDev c, T *bucket, size_t n, size
             }
     }
     if (__syncthreads_or(!ok)) {  // a peer died: nobody trains on a partial sum
-        for (size_t e = lo * EL + threadIdx.x; e < hi * EL && e < n; e += kCommThreads) poison_elem(bucket, e);
-        part = __longlong_as_double(0x7ff8000000000000ll);
+        poison_range<EL>(bucket, lo, hi, n);
+        part = poisoned_sumsq();
     }
-    if (sumsq_out) {
-        double tot = block_sum(part);
-        if (threadIdx.x == 0 && tot != 0.0) atomicAdd(sumsq_out, tot);
-    }
-    comm_end(c, s);
+    data_cta_end(c, s, part, sumsq_out);
 }
 
 // ---------------------------------------------------------------------------------------------------------------------
@@ -497,11 +497,7 @@ allreduce_twoshot_kernel(const __grid_constant__ CommDev c, T *bucket, size_t n,
     typedef Wire<kWire> W;
     constexpr int E = W::kElems;
     const uint32_t s = comm_begin(c);
-    if ((int)blockIdx.x >= n_data) {
-        metric_cta<false>(c, s, M);
-        comm_end(c, s);
-        return;
-    }
+    if (ran_metric_cta<false>(c, s, n_data, M)) return;
     const int half = s & 1;
     const size_t per = (S + n_data - 1) / n_data;
     const size_t lo = (size_t)blockIdx.x * per;
@@ -576,13 +572,9 @@ allreduce_twoshot_kernel(const __grid_constant__ CommDev c, T *bucket, size_t n,
         }
     } else {
         for (int q = 0; q < c.world; ++q) poison_range<E>(bucket, (size_t)q * S + lo, min((size_t)q * S + hi, nvec), n);
-        part = __longlong_as_double(0x7ff8000000000000ll);
+        part = poisoned_sumsq();
     }
-    if (sumsq_out) {
-        double tot = block_sum(part);
-        if (threadIdx.x == 0 && tot != 0.0) atomicAdd(sumsq_out, tot);
-    }
-    comm_end(c, s);
+    data_cta_end(c, s, part, sumsq_out);
 }
 
 __global__ void __launch_bounds__(kCommThreads) barrier_kernel(const __grid_constant__ CommDev c) {
@@ -600,76 +592,87 @@ constexpr size_t kNvlsMinBytes = 8 << 20;
 constexpr int kNvlsMinWorld = 8;
 static_assert(sizeof(dmlb_step_metrics) == 1880, "dmlb_step_metrics layout (dmlcloud_b200/_native.py StepMetrics mirrors it)");
 
-// The launch half of dmlb_comm_allreduce / dmlb_comm_allreduce_bf16 (arguments already checked).  T = float: the wire is
-// the caller's; T = __nv_bfloat16: always the bf16 wire.
+// bytes of a message of n elements: whole 16-byte wire vectors
+static size_t wire_bytes(size_t n, int wire) {
+    const size_t E = wire == DMLB_WIRE_BF16 ? 8 : 4;
+    return (n + E - 1) / E * 16;
+}
+
+// How one all-reduce runs.  algo: 0 picks the protocol, 1 one-shot, 2 two-shot, 3 NVLS, 4 NVLS reduce-scatter only,
+// 5 the barrier one-shot (never LL).
+enum class Proto { LL, Oneshot, Twoshot, Nvls, NvlsRsOnly };
+struct Plan {
+    Proto proto;
+    size_t items;  // what the data CTAs are spread over: LL lines, wire vectors (one-shot) or the vectors of one slice
+    size_t want;   // data CTAs the message asks for, before the co-residency cap
+};
+
+template <int v>
+using Int = std::integral_constant<int, v>;
+
+// The launch half of dmlb_comm_allreduce / dmlb_comm_allreduce_bf16 (arguments already checked): the plan, then one
+// launch.  T = float: the wire is the caller's; T = __nv_bfloat16: always the bf16 wire, the only one instantiated for
+// it.  DMLB_ESTATE: algo 3 or 4 on a communicator without a multicast mapping.
 template <class T>
-static int allreduce_launch(Comm *c, T *bucket, size_t n, int wire, float scale, double *sumsq, int algo,
+static int allreduce_launch(const CommDev &d, T *bucket, size_t n, int wire, float scale, double *sumsq, int algo,
                             const dmlb_step_metrics *metrics, cudaStream_t st) {
-    constexpr bool kF32Bucket = std::is_same<T, float>::value;
-    static_assert(kF32Bucket || kBf16Bucket<T>, "bucket element type");
-    const int W = c->dev.world;
-    const int E = wire == DMLB_WIRE_BF16 ? 8 : 4;
-    const size_t nvec = (n + E - 1) / E;
-    const size_t bytes = nvec * 16;
-    static const dmlb_step_metrics kNoMetrics = {};
-    const bool nvls = W > 1 && c->dev.mc != nullptr &&
+    static_assert(std::is_same<T, float>::value || kBf16Bucket<T>, "bucket element type");
+    const int W = d.world;
+    const size_t bytes = wire_bytes(n, wire), nvec = bytes / 16;
+    const bool nvls = W > 1 && d.mc != nullptr &&
                       (algo == 3 || algo == 4 || (algo == 0 && W >= kNvlsMinWorld && bytes >= kNvlsMinBytes));
     if ((algo == 3 || algo == 4) && !nvls && W > 1) return DMLB_ESTATE;
-    const bool nvls_rs_only = nvls && algo == 4;
     const bool oneshot = !nvls && (W == 1 || algo == 1 || algo == 5 || (algo == 0 && (bytes <= kOneshotMaxBytes || W <= 2)));
+    const int kU = W <= 2 ? 4 : (W <= 4 ? 2 : 1);
+    Plan p;
     // small messages at W > 1: the LL protocol (no barrier, no peer loads); algo 5 forces the barrier one-shot for A/B runs
     if (oneshot && W > 1 && algo != 5 && bytes <= kLLMaxPayload) {
         const int EL = wire == DMLB_WIRE_BF16 ? 4 : 2;
         const size_t n_lines = (n + EL - 1) / EL;
         size_t want = (n_lines + kCommThreads - 1) / kCommThreads;  // one line per thread while the grid can grow
-        const size_t cap = (size_t)min(kMaxCtas, sm_count() * 2) - 1;
-        if (want > cap) want = cap;
-        const int n_data = n == 0 ? 0 : (int)(want < 1 ? 1 : want);
-        const int grid = n_data + (metrics ? 1 : 0);
-        const dmlb_step_metrics &Mll = metrics ? *metrics : kNoMetrics;
-        if (wire == DMLB_WIRE_BF16)
-            allreduce_ll_kernel<T, DMLB_WIRE_BF16><<<grid, kCommThreads, 0, st>>>(c->dev, bucket, n, n_lines, scale, sumsq,
-                                                                                  n_data, Mll);
-        else if constexpr (kF32Bucket)
-            allreduce_ll_kernel<T, DMLB_WIRE_F32><<<grid, kCommThreads, 0, st>>>(c->dev, bucket, n, n_lines, scale, sumsq,
-                                                                                 n_data, Mll);
-        return launched();
+        p = {Proto::LL, n_lines, want};
+    } else {
+        const size_t items = oneshot ? nvec : (nvec + W - 1) / W;  // vectors a CTA grid is spread over
+        size_t want = (items + (size_t)kCommThreads * kU - 1) / ((size_t)kCommThreads * kU);
+        p = {oneshot ? Proto::Oneshot : !nvls ? Proto::Twoshot : algo == 4 ? Proto::NvlsRsOnly : Proto::Nvls, items, want};
     }
-    const int kU = W <= 2 ? 4 : (W <= 4 ? 2 : 1);
-    const size_t items = oneshot ? nvec : (nvec + W - 1) / W;  // vectors a CTA grid is spread over
-    size_t want = (items + (size_t)kCommThreads * kU - 1) / ((size_t)kCommThreads * kU);
     // all CTAs co-resident (the per-CTA barriers need that); one slot is kept for the metric CTA
     size_t cap = (size_t)min(kMaxCtas, sm_count() * 2) - 1;
-    if (want > cap) want = cap;
-    const int n_data = n == 0 ? 0 : (int)(want < 1 ? 1 : want);
+    const int n_data = n == 0 ? 0 : (int)(p.want > cap ? cap : (p.want < 1 ? 1 : p.want));
     const int grid = n_data + (metrics ? 1 : 0);
+    static const dmlb_step_metrics kNoMetrics = {};
     const dmlb_step_metrics &M = metrics ? *metrics : kNoMetrics;
-#define DMLB_LAUNCH_AR(WIRE, U)                                                                                          \
-    do {                                                                                                                 \
-        if (oneshot)                                                                                                     \
-            allreduce_oneshot_kernel<T, WIRE, U><<<grid, kCommThreads, 0, st>>>(c->dev, bucket, n, nvec, scale, sumsq,   \
-                                                                                n_data, M);                              \
-        else if (nvls_rs_only)                                                                                           \
-            allreduce_twoshot_kernel<T, WIRE, U, 2><<<grid, kCommThreads, 0, st>>>(c->dev, bucket, n, nvec, items,     \
-                                                                                   scale, sumsq, n_data, M);             \
-        else if (nvls)                                                                                                   \
-            allreduce_twoshot_kernel<T, WIRE, U, 1><<<grid, kCommThreads, 0, st>>>(c->dev, bucket, n, nvec, items,     \
-                                                                                   scale, sumsq, n_data, M);             \
-        else                                                                                                             \
-            allreduce_twoshot_kernel<T, WIRE, U, 0><<<grid, kCommThreads, 0, st>>>(c->dev, bucket, n, nvec, items,     \
-                                                                                   scale, sumsq, n_data, M);             \
-    } while (0)
-    if (wire == DMLB_WIRE_BF16) {
-        if (kU == 4) DMLB_LAUNCH_AR(DMLB_WIRE_BF16, 4);
-        else if (kU == 2) DMLB_LAUNCH_AR(DMLB_WIRE_BF16, 2);
-        else DMLB_LAUNCH_AR(DMLB_WIRE_BF16, 1);
-    } else if constexpr (kF32Bucket) {
-        if (kU == 4) DMLB_LAUNCH_AR(DMLB_WIRE_F32, 4);
-        else if (kU == 2) DMLB_LAUNCH_AR(DMLB_WIRE_F32, 2);
-        else DMLB_LAUNCH_AR(DMLB_WIRE_F32, 1);
-    }
-#undef DMLB_LAUNCH_AR
+    const auto launch = [&](auto wire_c, auto u_c) {
+        constexpr int kWire = decltype(wire_c)::value, U = decltype(u_c)::value;
+        const auto go = [&](auto kernel, auto... sizes) {  // sizes: what the kernel takes between n and scale
+            kernel<<<grid, kCommThreads, 0, st>>>(d, bucket, n, sizes..., scale, sumsq, n_data, M);
+        };
+        switch (p.proto) {
+        case Proto::LL: return go(allreduce_ll_kernel<T, kWire>, p.items);
+        case Proto::Oneshot: return go(allreduce_oneshot_kernel<T, kWire, U>, nvec);
+        case Proto::Twoshot: return go(allreduce_twoshot_kernel<T, kWire, U, 0>, nvec, p.items);
+        case Proto::Nvls: return go(allreduce_twoshot_kernel<T, kWire, U, 1>, nvec, p.items);
+        case Proto::NvlsRsOnly: return go(allreduce_twoshot_kernel<T, kWire, U, 2>, nvec, p.items);
+        }
+    };
+    const auto launch_ku = [&](auto wire_c) {
+        kU == 4 ? launch(wire_c, Int<4>()) : kU == 2 ? launch(wire_c, Int<2>()) : launch(wire_c, Int<1>());
+    };
+    if (wire == DMLB_WIRE_BF16) launch_ku(Int<DMLB_WIRE_BF16>());
+    else if constexpr (!kBf16Bucket<T>) launch_ku(Int<DMLB_WIRE_F32>());
     return launched();
+}
+
+// What both all-reduce entry points refuse.  Nothing is launched for an empty bucket unless a step exchange rides on it.
+static int check_allreduce(void *comm, const void *bucket, size_t n, int wire, const dmlb_step_metrics *metrics,
+                           bool &empty) {
+    if (!comm || (!bucket && n)) return DMLB_EINVAL;
+    if (wire != DMLB_WIRE_F32 && wire != DMLB_WIRE_BF16) return DMLB_EINVAL;
+    if ((uintptr_t)bucket & 15) return DMLB_EALIGN;
+    empty = n == 0 && !metrics;
+    const Comm *c = reinterpret_cast<const Comm *>(comm);
+    if (c->dev.world > 1 && wire_bytes(n, wire) > c->dev.msg_cap) return DMLB_ECAPACITY;
+    return DMLB_OK;
 }
 
 }  // namespace dmlb
@@ -724,14 +727,9 @@ int dmlb_comm_set_multicast(void *comm, void *mc_base) {
 
 int dmlb_comm_allreduce(void *comm, float *bucket, size_t n, int wire, float scale, double *sumsq, int algo,
                         const dmlb_step_metrics *metrics, void *stream) {
-    if (!comm || (!bucket && n)) return DMLB_EINVAL;
-    if (wire != DMLB_WIRE_F32 && wire != DMLB_WIRE_BF16) return DMLB_EINVAL;
-    if ((uintptr_t)bucket & 15) return DMLB_EALIGN;
-    if (n == 0 && !metrics) return DMLB_OK;
-    Comm *c = reinterpret_cast<Comm *>(comm);
-    const int E = wire == DMLB_WIRE_BF16 ? 8 : 4;
-    const size_t bytes = (n + E - 1) / E * 16;
-    if (c->dev.world > 1 && bytes > c->dev.msg_cap) return DMLB_ECAPACITY;
+    bool empty;
+    const int rc = check_allreduce(comm, bucket, n, wire, metrics, empty);
+    if (rc != DMLB_OK || empty) return rc;
     if (metrics) {
         const dmlb_step_metrics &m = *metrics;
         if (!m.acc || !m.cnt || !m.desc || !m.counter || !m.out_ring || m.ring_slots < 1 || m.capacity < 1)
@@ -752,17 +750,15 @@ int dmlb_comm_allreduce(void *comm, float *bucket, size_t n, int wire, float sca
         }
         if (!folds_disjoint(m.folds, m.n_folds)) return DMLB_EINVAL;
     }
-    return allreduce_launch(c, bucket, n, wire, scale, sumsq, algo, metrics, (cudaStream_t)stream);
+    return allreduce_launch(reinterpret_cast<Comm *>(comm)->dev, bucket, n, wire, scale, sumsq, algo, metrics, (cudaStream_t)stream);
 }
 
 int dmlb_comm_allreduce_bf16(void *comm, uint16_t *bucket, size_t n, float scale, double *sumsq, int algo, void *stream) {
-    if (!comm || (!bucket && n)) return DMLB_EINVAL;
-    if ((uintptr_t)bucket & 15) return DMLB_EALIGN;
-    if (n == 0) return DMLB_OK;
-    Comm *c = reinterpret_cast<Comm *>(comm);
-    if (c->dev.world > 1 && (n + 7) / 8 * 16 > c->dev.msg_cap) return DMLB_ECAPACITY;
-    return allreduce_launch(c, reinterpret_cast<__nv_bfloat16 *>(bucket), n, DMLB_WIRE_BF16, scale, sumsq, algo, nullptr,
-                            (cudaStream_t)stream);
+    bool empty;
+    const int rc = check_allreduce(comm, bucket, n, DMLB_WIRE_BF16, nullptr, empty);
+    if (rc != DMLB_OK || empty) return rc;
+    return allreduce_launch(reinterpret_cast<Comm *>(comm)->dev, reinterpret_cast<__nv_bfloat16 *>(bucket), n, DMLB_WIRE_BF16,
+                            scale, sumsq, algo, nullptr, (cudaStream_t)stream);
 }
 
 int dmlb_comm_error(void *comm, int *error) {

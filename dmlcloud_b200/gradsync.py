@@ -16,6 +16,7 @@ Per bucket it picks one of three routes, all of them running libdmlb kernels on 
 A bf16 bucket (DDP's bucket of bf16 parameters) is already in wire format: it always travels as bf16, whatever `wire`
 says, through the same three routes (dmlb_comm_allreduce_bf16 / dmlb_bucket_scale_bf16 + all_reduce / in place).
 """
+import collections
 import ctypes
 import warnings
 
@@ -25,6 +26,24 @@ import torch.distributed as dist
 from . import _native as N
 
 WIRES = {'fp32': N.WIRE_F32, 'bf16': N.WIRE_BF16}
+
+# The in-place kernels of one gradient element type (a bf16 gradient is stored back rounded to nearest even):
+# scale(lib, ptr, n, s, stream), sumsq(lib, ptr, n, sumsq_ptr, stream), clip(lib, ptr, n, sumsq_ptr, max_norm, stream)
+_Kernels = collections.namedtuple('_Kernels', 'scale sumsq clip')
+_KERNELS = {
+    torch.float32: _Kernels(lambda lib, p, n, s, st: lib.dmlb_bucket_scale_f32(p, n, s, st),
+                            lambda lib, p, n, sq, st: lib.dmlb_bucket_sumsq_f32(p, n, sq, st),
+                            lambda lib, p, n, sq, m, st: lib.dmlb_bucket_clip_f32(p, n, sq, m, st)),
+    torch.bfloat16: _Kernels(lambda lib, p, n, s, st: lib.dmlb_bucket_scale_bf16(p, n, s, st),
+                             lambda lib, p, n, sq, st: lib.dmlb_bucket_sumsq_bf16(p, n, sq, st),
+                             lambda lib, p, n, sq, m, st: lib.dmlb_bucket_clip_bf16(p, n, sq, m, st)),
+}
+
+
+def wire_bytes(n, wire):
+    """Bytes of an n-element message on `wire` ('fp32' | 'bf16'): whole 16-byte vectors of 4 or 8 elements."""
+    per = 8 if wire == 'bf16' else 4
+    return ((n + per - 1) // per) * 16
 
 
 class PeerComm:
@@ -250,8 +269,8 @@ class PeerComm:
             warnings.warn(f'peer-memory communicator unavailable ({exc}); using the NCCL route')
             return None
 
-    def fits(self, wire_bytes):
-        return self.world == 1 or wire_bytes <= self.max_message_bytes
+    def fits(self, nbytes):
+        return self.world == 1 or nbytes <= self.max_message_bytes
 
     def failed(self):
         """True once a collective on this communicator has timed out waiting for a peer.  A plain read of mapped pinned
@@ -405,36 +424,42 @@ class GradBucketSync:
         return fut
 
     def _reduce_bucket(self, buf, index=0):
-        if buf.dtype not in (torch.float32, torch.bfloat16) or not buf.is_contiguous():
+        """A bf16 bucket travels on the bf16 wire whatever `self.wire` says (it is its own wire format): result =
+        bf16_rn(sum over ranks, fp32 in rank order, of bf16_rn(g_r * 1/W)); sumsq over the stored bf16 values."""
+        if buf.dtype not in _KERNELS or not buf.is_contiguous():
             raise RuntimeError(f'GradBucketSync expects contiguous fp32 or bf16 gradient buckets, got a '
                                f'{"" if buf.is_contiguous() else "non-contiguous "}{buf.dtype} bucket')
-        if buf.dtype == torch.bfloat16:
-            return self._reduce_bucket_bf16(buf, index)
         lib = N.cuda_lib(self.device.index)  # runs on the autograd thread: per-thread device of libdmlb's runtime
-        n = buf.numel()
-        wire = WIRES[self.wire]
-        wire_bytes = ((n + 7) // 8) * 16 if self.wire == 'bf16' else ((n + 3) // 4) * 16
+        n, ptr, k = buf.numel(), buf.data_ptr(), _KERNELS[buf.dtype]
+        bf16_bucket = buf.dtype == torch.bfloat16
+        wire = 'bf16' if bf16_bucket else self.wire
+        cast = wire == 'bf16' and not bf16_bucket  # an fp32 bucket cast to the bf16 wire and back
         sumsq_ptr = self.sumsq.data_ptr() if self.sumsq is not None else None
         self.buckets_seen += 1
         self.buckets_this_step += 1
 
         if self.world == 1:
             st = N.stream_ptr()
-            if self.wire == 'bf16':  # K1 and K2 collapse into one in-place launch when there is nobody to exchange with
-                N.check(lib.dmlb_bucket_round_bf16_f32(buf.data_ptr(), n, self.scale, sumsq_ptr, st), 'round_bf16')
+            if cast:  # K1 and K2 collapse into one in-place launch when there is nobody to exchange with
+                N.check(lib.dmlb_bucket_round_bf16_f32(ptr, n, self.scale, sumsq_ptr, st), 'round_bf16')
             else:
-                N.check(lib.dmlb_bucket_scale_f32(buf.data_ptr(), n, self.scale, st), 'scale')
+                if not bf16_bucket:  # (the average of one bf16 bucket is the bucket itself: 1/W = 1 multiplies exactly)
+                    N.check(k.scale(lib, ptr, n, self.scale, st), 'scale')
                 if sumsq_ptr:
-                    N.check(lib.dmlb_bucket_sumsq_f32(buf.data_ptr(), n, sumsq_ptr, st), 'sumsq')
+                    N.check(k.sumsq(lib, ptr, n, sumsq_ptr, st), 'sumsq')
             self.last_routes[index] = 'single'
             return self._done(buf)
 
-        if self.comm is not None and self.comm.fits(wire_bytes) and buf.data_ptr() % 16 == 0:
-            cur = torch.cuda.current_stream(self.device)
-            self.comm_stream.wait_stream(cur)
+        if self.comm is not None and self.comm.fits(wire_bytes(n, wire)) and ptr % 16 == 0:
+            self.comm_stream.wait_stream(torch.cuda.current_stream(self.device))
             with torch.cuda.stream(self.comm_stream):
-                N.check(lib.dmlb_comm_allreduce(self.comm.handle, buf.data_ptr(), n, wire, self.scale, sumsq_ptr,
-                                                self.algo, None, N.stream_ptr(self.comm_stream)), 'comm_allreduce')
+                st = N.stream_ptr(self.comm_stream)
+                if bf16_bucket:
+                    rc = lib.dmlb_comm_allreduce_bf16(self.comm.handle, ptr, n, self.scale, sumsq_ptr, self.algo, st)
+                else:
+                    rc = lib.dmlb_comm_allreduce(self.comm.handle, ptr, n, WIRES[wire], self.scale, sumsq_ptr, self.algo,
+                                                 None, st)
+                N.check(rc, 'comm_allreduce')
                 buf.record_stream(self.comm_stream)
                 fut = self._done(buf)
             self.last_routes[index] = 'peer'
@@ -443,67 +468,24 @@ class GradBucketSync:
         # NCCL route: K1 -> all_reduce -> K2
         self.last_routes[index] = 'nccl'
         st = N.stream_ptr()
-        if self.wire == 'fp32':
-            N.check(lib.dmlb_bucket_scale_f32(buf.data_ptr(), n, self.scale, st), 'scale')
+        if cast:  # through a bf16 staging buffer, unpacked back into the bucket (+ its sum of squares)
+            stage = self._stage_for(index, n)[:n]
+            N.check(lib.dmlb_bucket_pack_f32_bf16(ptr, stage.data_ptr(), n, self.scale, st), 'pack')
+            fut = dist.all_reduce(stage, group=self.group, async_op=True).get_future()
+
+            def finish(f):
+                N.check(N.cuda_lib(self.device.index).dmlb_bucket_unpack_bf16_f32(
+                    f.value()[0].data_ptr(), ptr, n, 1.0, sumsq_ptr, N.stream_ptr()), 'unpack')
+                return buf
+        else:  # scaled in place in the bucket's own type, then the sum of squares of the result
+            N.check(k.scale(lib, ptr, n, self.scale, st), 'scale')
             fut = dist.all_reduce(buf, group=self.group, async_op=True).get_future()
 
-            def finish_f32(f):
+            def finish(f):
                 out = f.value()[0]
                 if sumsq_ptr:
-                    N.check(N.cuda_lib(self.device.index).dmlb_bucket_sumsq_f32(out.data_ptr(), n, sumsq_ptr,
-                                                                                 N.stream_ptr()), 'sumsq')
+                    N.check(k.sumsq(N.cuda_lib(self.device.index), out.data_ptr(), n, sumsq_ptr, N.stream_ptr()), 'sumsq')
                 return out
-
-            return fut.then(finish_f32)
-
-        stage = self._stage_for(index, n)[:n]
-        N.check(lib.dmlb_bucket_pack_f32_bf16(buf.data_ptr(), stage.data_ptr(), n, self.scale, st), 'pack')
-        fut = dist.all_reduce(stage, group=self.group, async_op=True).get_future()
-
-        def finish_bf16(f):
-            reduced = f.value()[0]
-            N.check(N.cuda_lib(self.device.index).dmlb_bucket_unpack_bf16_f32(
-                reduced.data_ptr(), buf.data_ptr(), n, 1.0, sumsq_ptr, N.stream_ptr()), 'unpack')
-            return buf
-
-        return fut.then(finish_bf16)
-
-    def _reduce_bucket_bf16(self, buf, index):
-        """A bf16 bucket: bf16 wire always (it is the bucket's own format; `self.wire` governs fp32 buckets only).
-        Result = bf16_rn(sum over ranks, fp32 in rank order, of bf16_rn(g_r * 1/W)); sumsq over the stored bf16 values."""
-        lib = N.cuda_lib(self.device.index)
-        n = buf.numel()
-        sumsq_ptr = self.sumsq.data_ptr() if self.sumsq is not None else None
-        self.buckets_seen += 1
-        self.buckets_this_step += 1
-
-        if self.world == 1:  # the average of one rank is the bucket itself (1/W = 1 multiplies exactly)
-            if sumsq_ptr:
-                N.check(lib.dmlb_bucket_sumsq_bf16(buf.data_ptr(), n, sumsq_ptr, N.stream_ptr()), 'sumsq_bf16')
-            self.last_routes[index] = 'single'
-            return self._done(buf)
-
-        if self.comm is not None and self.comm.fits(((n + 7) // 8) * 16) and buf.data_ptr() % 16 == 0:
-            self.comm_stream.wait_stream(torch.cuda.current_stream(self.device))
-            with torch.cuda.stream(self.comm_stream):
-                N.check(lib.dmlb_comm_allreduce_bf16(self.comm.handle, buf.data_ptr(), n, self.scale, sumsq_ptr,
-                                                     self.algo, N.stream_ptr(self.comm_stream)), 'comm_allreduce_bf16')
-                buf.record_stream(self.comm_stream)
-                fut = self._done(buf)
-            self.last_routes[index] = 'peer'
-            return fut
-
-        # NCCL route: scale in place -> all_reduce (bf16) -> sum of squares of the result
-        self.last_routes[index] = 'nccl'
-        N.check(lib.dmlb_bucket_scale_bf16(buf.data_ptr(), n, self.scale, N.stream_ptr()), 'scale_bf16')
-        fut = dist.all_reduce(buf, group=self.group, async_op=True).get_future()
-
-        def finish(f):
-            out = f.value()[0]
-            if sumsq_ptr:
-                N.check(N.cuda_lib(self.device.index).dmlb_bucket_sumsq_bf16(out.data_ptr(), n, sumsq_ptr,
-                                                                              N.stream_ptr()), 'sumsq_bf16')
-            return out
 
         return fut.then(finish)
 
@@ -520,29 +502,22 @@ def clip_grad_norm_(parameters, max_norm, sumsq=None):
     rescaled as bf16_rn(g * coef).
     If `sumsq` (a 1-element fp64 CUDA tensor already holding sum g^2 of exactly these parameters, e.g. accumulated by the
     fused all-reduce) is given, the first pass is skipped.  Returns the 0-d CUDA tensor holding the total norm."""
-    grads = [_flat(p.grad) for p in parameters if p.grad is not None]
+    grads = [(_flat(p.grad), _KERNELS[p.grad.dtype]) for p in parameters if p.grad is not None]
     if not grads:
         return torch.tensor(0.0)
-    device = grads[0].device
+    device = grads[0][0].device
     lib = N.cuda_lib(device.index)
     st = N.stream_ptr()
     if sumsq is None:
         sumsq = torch.zeros(1, dtype=torch.float64, device=device)
-        for g in grads:
-            if g.dtype == torch.bfloat16:
-                N.check(lib.dmlb_bucket_sumsq_bf16(g.data_ptr(), g.numel(), sumsq.data_ptr(), st), 'sumsq_bf16')
-            else:
-                N.check(lib.dmlb_bucket_sumsq_f32(g.data_ptr(), g.numel(), sumsq.data_ptr(), st), 'sumsq')
-    for g in grads:
-        if g.dtype == torch.bfloat16:
-            N.check(lib.dmlb_bucket_clip_bf16(g.data_ptr(), g.numel(), sumsq.data_ptr(), float(max_norm), st),
-                    'clip_bf16')
-        else:
-            N.check(lib.dmlb_bucket_clip_f32(g.data_ptr(), g.numel(), sumsq.data_ptr(), float(max_norm), st), 'clip')
+        for g, k in grads:
+            N.check(k.sumsq(lib, g.data_ptr(), g.numel(), sumsq.data_ptr(), st), 'sumsq')
+    for g, k in grads:
+        N.check(k.clip(lib, g.data_ptr(), g.numel(), sumsq.data_ptr(), float(max_norm), st), 'clip')
     return sumsq.sqrt().to(torch.float32).reshape(())
 
 
 def _flat(g):
-    if g.dtype not in (torch.float32, torch.bfloat16) or not g.is_contiguous():
+    if g.dtype not in _KERNELS or not g.is_contiguous():
         raise RuntimeError('clip_grad_norm_ (dmlcloud_b200) expects contiguous fp32 or bf16 gradients')
     return g

@@ -48,7 +48,7 @@ from torch.nn.parallel import DistributedDataParallel
 from torch.utils._pytree import tree_flatten, tree_unflatten
 
 from . import _native as N
-from .gradsync import WIRES, PeerComm
+from .gradsync import WIRES, PeerComm, wire_bytes
 from .metrics import HostFeed, StepRing, _RingResult
 
 
@@ -156,7 +156,7 @@ class GraphedTrainStep:
             comm = pipeline.metric_comm  # no gradients to exchange: the metric records ride on the metric communicator
         if comm is None and self.world == 1:
             comm = self._own_comm = PeerComm(self.device, max_message_bytes=1 << 16)  # local: no peers, no mapping
-        if comm is None or (self.needs_sync and not comm.fits(self._wire_bytes(self.bucket.total))):
+        if comm is None or (self.needs_sync and not comm.fits(wire_bytes(self.bucket.total, self.wire))):
             raise RuntimeError('cuda_graph mode needs the peer-memory communicator (grad_route "auto"/"peer") and a '
                                'gradient set that fits grad_arena_bytes')
         self.comm = comm
@@ -194,9 +194,6 @@ class GraphedTrainStep:
     @property
     def static(self):
         return self.first.batch if self.first is not None else None
-
-    def _wire_bytes(self, n):
-        return ((n + 7) // 8) * 16 if self.wire == 'bf16' else ((n + 3) // 4) * 16
 
     def _say(self, what, message):
         if what not in self._said:

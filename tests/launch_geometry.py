@@ -21,7 +21,7 @@ PINS = [
     ('bucket_kernels.cu', 'size_t g = want < sms ? (want < 1 ? 1 : want) : ((want + sms - 1) / sms) * sms;'),
     ('bucket_kernels.cu', 'if (g > cap) g = cap;'),
     ('bucket_kernels.cu', 'chunk = (nvec + g - 1) / g;'),
-    ('bucket_kernels.cu', 'grid = stream_grid(nvec, unroll_of<F>::value, kCtasPerSm);'),
+    ('bucket_kernels.cu', 'grid = stream_grid(nvec, kUnroll, kCtasPerSm);'),
     ('optim_kernels.cu', 'const int grid = stream_grid(n / 4, 2, 2);'),
     ('optim_kernels.cu', 'const int grid = stream_grid(n, 1, 2);'),
     ('peer_comm.cuh', 'constexpr int kMaxCtas = 264;  // 2 per SM on 132 SMs (launches use at most 2 x the device\'s SM count)'),
