@@ -41,6 +41,17 @@ class Range(Structure):
     _fields_ = [('begin', c_int32), ('end', c_int32)]
 
 
+class ImageNorm(Structure):
+    """dmlb_image_norm: per-channel mean and std of dmlb_image_batch_u8 (channels past C are ignored)."""
+    _fields_ = [('mean', c_float * 4), ('std', c_float * 4)]
+
+    @classmethod
+    def of(cls, mean, std):
+        """From per-channel sequences of length C <= 4 (the unused channels get mean 0, std 1)."""
+        mean, std = [float(m) for m in mean], [float(s) for s in std]
+        return cls(tuple(mean + [0.0] * (4 - len(mean))), tuple(std + [1.0] * (4 - len(std))))
+
+
 class StepMetrics(Structure):
     """dmlb_step_metrics: descriptor of the per-step metric exchange fused into the gradient all-reduce."""
     _fields_ = [('acc', c_void_p), ('cnt', c_void_p), ('desc', c_void_p), ('counter', c_void_p), ('out_ring', c_void_p),
@@ -116,6 +127,9 @@ SIGNATURES = {
     'dmlb_shard_gather_u8': (c_int, [c_void_p, c_void_p, c_int64, c_int64, c_float, c_float, c_void_p, c_int, c_void_p]),
     'dmlb_shard_gather_i64': (c_int, [c_void_p, c_void_p, c_int64, c_void_p, c_void_p]),
     'dmlb_shard_slice': (c_int, [c_void_p, c_int64, c_int64, c_int64, c_int64, c_void_p, c_void_p]),
+    'dmlb_image_batch_u8': (c_int, [c_void_p, c_void_p, c_int64, c_int32, c_int32, c_int32, c_int32, c_int32, c_int32,
+                                    c_int, c_int, c_uint64, c_int64, POINTER(ImageNorm), c_void_p, c_int, c_int,
+                                    c_void_p, c_void_p]),
 }
 
 _lib = None

@@ -12,6 +12,8 @@ batches through instead of falling into the general path.
 
 New (SURVEY §8f-1): `DeviceShardedDataset` keeps the whole uint8 dataset in HBM and produces each batch with one
 gather + normalise kernel (libdmlb dmlb_shard_gather_u8) instead of a host DataLoader + H2D copy per step.
+`DeviceImageDataset` does the same for colour images (HWC uint8) with pad / random or centre crop / horizontal flip /
+per-channel normalisation in one kernel (dmlb_image_batch_u8).
 """
 from concurrent.futures import ThreadPoolExecutor
 from typing import Iterable, Sequence
@@ -263,5 +265,92 @@ class DeviceShardedDataset:
                                              self.std, x.data_ptr(), int(self.out_dtype == torch.bfloat16), st),
                     'shard_gather_u8')
             N.check(lib.dmlb_shard_gather_i64(self.labels.data_ptr(), view.data_ptr(), b, y.data_ptr(), st),
+                    'shard_gather_i64')
+            yield x, y
+
+
+class DeviceImageDataset(DeviceShardedDataset):
+    """Device-resident colour-image dataset with the usual training augmentation (SURVEY §8f-1).
+
+    images: uint8 [N, H, W, C] (HWC, C <= 4), labels: int64 [N].  Each batch is one libdmlb launch
+    (dmlb_image_batch_u8) plus the label gather, and equals, bit for bit, torchvision's
+        pad(padding, fill=0) -> crop (random or centre) -> hflip (probability 1/2) -> to_tensor -> normalize(mean, std)
+    on every sample.  x is [B, C, h, w] in `memory_format` (torch.contiguous_format or torch.channels_last), in
+    `out_dtype` (float32 or bfloat16).  crop: None (the whole padded image), an int or (h, w).  random_crop=False takes
+    the centre window (validation).  A sample's window and flip depend only on (aug_seed, epoch, its dataset index), so
+    they are the same at every rank and world size; set_epoch advances the shard permutation and the augmentation
+    together.  Sharding, shuffle, even_shards and drop_last are DeviceShardedDataset's.
+    """
+
+    def __init__(self, images, labels, batch_size, mean, std, crop=None, padding=0, random_crop=True, hflip=False,
+                 memory_format=torch.contiguous_format, out_dtype=torch.float32, shuffle=True, even_shards=True, seed=0,
+                 aug_seed=None, rank=None, world_size=None, device=None, drop_last=False):
+        if images.dim() != 4 or not 1 <= images.shape[3] <= 4:
+            raise ValueError('images must be uint8 [N, H, W, C] with 1 <= C <= 4')
+        if memory_format not in (torch.contiguous_format, torch.channels_last):
+            raise ValueError('memory_format must be torch.contiguous_format or torch.channels_last')
+        super().__init__(images, labels, batch_size, shuffle=shuffle, even_shards=even_shards, seed=seed, rank=rank,
+                         world_size=world_size, device=device, out_dtype=out_dtype, drop_last=drop_last)
+        H, W, C = self.item_shape
+        mean, std = [float(m) for m in mean], [float(s) for s in std]
+        if len(mean) != C or len(std) != C:
+            raise ValueError(f'mean and std need one value per channel ({C})')
+        if any(s == 0.0 for s in std):
+            raise ValueError('std must not be 0')
+        self.mean, self.std = mean, std
+        self.padding = int(padding)
+        if crop is None:
+            crop = (H + 2 * self.padding, W + 2 * self.padding)
+        self.crop = (int(crop), int(crop)) if isinstance(crop, int) else tuple(int(c) for c in crop)
+        if self.padding < 0 or not (0 < self.crop[0] <= H + 2 * self.padding and 0 < self.crop[1] <= W + 2 * self.padding):
+            raise ValueError(f'crop {self.crop} does not fit the {H}x{W} images padded by {self.padding}')
+        self.random_crop, self.hflip = bool(random_crop), bool(hflip)
+        self.memory_format = memory_format
+        self.aug_seed = seed if aug_seed is None else aug_seed
+        self._norm = self._N.ImageNorm.of(mean, std)
+
+    def _launch(self, idx, x, params=None):
+        N = self._N
+        H, W, C = self.item_shape
+        lib = N.cuda_lib(self.device.index)
+        N.check(lib.dmlb_image_batch_u8(self.images.data_ptr(), idx.data_ptr(), idx.numel(), H, W, C, self.crop[0],
+                                        self.crop[1], self.padding, int(self.random_crop), int(self.hflip),
+                                        self.aug_seed % (1 << 64), self.epoch, self._norm, x.data_ptr(),
+                                        int(self.out_dtype == torch.bfloat16),
+                                        int(self.memory_format == torch.channels_last),
+                                        None if params is None else params.data_ptr(), N.stream_ptr()),
+                'image_batch_u8')
+
+    def _empty(self, b):
+        C = self.item_shape[2]
+        h, w = self.crop
+        if self.memory_format == torch.channels_last:
+            return torch.empty((b, h, w, C), dtype=self.out_dtype, device=self.device).permute(0, 3, 1, 2)
+        return torch.empty((b, C, h, w), dtype=self.out_dtype, device=self.device)
+
+    def augment_params(self):
+        """(indices, params): this rank's dataset indices for the current epoch in iteration order, and the int32
+        [count, 3] {top, left, flipped} of each (top/left in padded coordinates), as the batches of this epoch use them."""
+        idx = self.epoch_indices()
+        params = torch.empty((idx.numel(), 3), dtype=torch.int32, device=self.device)
+        for start in range(0, idx.numel(), self.batch_size):
+            view = idx[start:start + self.batch_size]
+            self._launch(view, self._empty(view.numel()), params[start:start + view.numel()])
+        return idx, params
+
+    def __iter__(self):
+        N = self._N
+        lib = N.cuda_lib(self.device.index)
+        idx = self.epoch_indices()
+        count = idx.numel()
+        for start in range(0, count, self.batch_size):
+            b = min(self.batch_size, count - start)
+            if b < self.batch_size and self.drop_last:
+                return
+            x = self._empty(b)
+            y = torch.empty(b, dtype=torch.int64, device=self.device)
+            view = idx[start:start + b]
+            self._launch(view, x)
+            N.check(lib.dmlb_shard_gather_i64(self.labels.data_ptr(), view.data_ptr(), b, y.data_ptr(), N.stream_ptr()),
                     'shard_gather_i64')
             yield x, y

@@ -363,6 +363,36 @@ int dmlb_shard_gather_i64(const int64_t *labels, const int64_t *idx, int64_t bat
 int dmlb_shard_slice(const int64_t *perm, int64_t first, int64_t count, int64_t rank, int64_t world, int64_t *idx_out,
                      void *stream);
 
+/* Colour-image batch: gather + zero pad + crop + horizontal flip + per-channel normalise, one launch.
+ *   images : uint8 [n, H, W, C] (HWC, as numpy / PIL store it), C in 1..4; row i of the batch is images[idx[i]]
+ *   out    : logical [batch, C, out_h, out_w], NCHW in memory (channels_last == 0) or NHWC (channels_last != 0), fp32 or
+ *            bf16 (out_bf16 != 0: RNE rounding of the fp32 value)
+ *   out[i, c, y, x] = ((float)P[top + y][left + x'][c] / 255.0f - mean[c]) / std[c]   in IEEE fp32, in that order,
+ *            P = the image with `pad` zero bytes on all four sides, x' = flipped ? out_w - 1 - x : x
+ *            == torchvision pad(fill=0) -> crop -> hflip -> to_tensor -> normalize, bit for bit.
+ * The window of a sample depends only on (seed, epoch, row = idx[i]), never on the batch, rank or world size:
+ *   mix(z)  = SplitMix64 finaliser: z = (z ^ z >> 30) * 0xbf58476d1ce4e5b9; z = (z ^ z >> 27) * 0x94d049bb133111eb;
+ *             z ^ z >> 31   (uint64 arithmetic, g = 0x9e3779b97f4a7c15)
+ *   h       = mix(mix(mix(seed + g) ^ (epoch + g)) ^ (row + g))
+ *   dy = H + 2 pad - out_h, dx = W + 2 pad - out_w
+ *   crop_mode 1 (random): top = ((h & 0xffffffff) * (dy + 1)) >> 32,  left = ((h >> 32) * (dx + 1)) >> 32
+ *   crop_mode 0 (centre): top = round(dy / 2), left = round(dx / 2), halves to even (torchvision center_crop)
+ *   flipped = hflip ? mix(h + g) >> 63 : 0
+ * params_out (optional, DEVICE int32 [batch][3]) receives {top, left, flipped} of every sample.
+ * DMLB_EINVAL (nothing launched): C outside 1..4, a window larger than the padded image, std[c] == 0 for c < C, a NULL
+ * norm, NULL images / idx / out with batch > 0, out_w * C above 49,136 bytes.  DMLB_EALIGN: out not aligned to its
+ * element.  Any images alignment works (16-byte loads when images is 16-byte aligned, byte loads otherwise); out is
+ * written with 16-byte stores between scalar heads and tails of every contiguous run.
+ * Algorithmic bytes/sample: window bytes inside the image read + out_h * out_w * C * (4 | 2) written. */
+typedef struct {
+    float mean[4];
+    float std[4];
+} dmlb_image_norm;
+int dmlb_image_batch_u8(const uint8_t *images, const int64_t *idx, int64_t batch, int32_t H, int32_t W, int32_t C,
+                        int32_t out_h, int32_t out_w, int32_t pad, int crop_mode, int hflip, uint64_t seed, int64_t epoch,
+                        const dmlb_image_norm *norm, void *out, int out_bf16, int channels_last, int32_t *params_out,
+                        void *stream);
+
 #ifdef __cplusplus
 }
 #endif
