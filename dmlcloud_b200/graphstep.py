@@ -39,6 +39,9 @@ step: both issue the same collective.  A step kind that issued a second collecti
 Requirements: FlatAdam / FlatSGD, or torch optimizers constructed with `capturable=True` and no scheduler; `step()` must
 not synchronise with the host (no .item(), no printing of tensors) and must depend on the batch only through its
 signature (shapes, dtypes, python values), as any captured code must.
+
+`GraphedValStep` does the same for the validation step (`TrainValStage.cuda_graph_val`): val_step and its metric folds,
+one graph per batch signature and module-mode snapshot, no gradients, no optimizer, no collective.
 """
 import ctypes
 
@@ -114,7 +117,62 @@ class _ShapeGraph:
         self.replays = 0
 
 
-class GraphedTrainStep:
+class _StaticBatchStep:
+    """What the captured training and validation steps share: warnings said once, and the copy of a batch into the static
+    inputs of its signature's graph (`_load`).  Subclasses set `stage`, `device`, `_said`, `_copy_stream`, `_staging`."""
+
+    STAGE_MIN_BYTES = 1 << 20
+
+    def _say(self, what, message):
+        if what not in self._said:
+            self._said.add(what)
+            self.stage.logger.warning(message)
+
+    def _load(self, key, shape, leaves):
+        """Bring the batch's leaves into the static input buffers of its own signature's graph.  Large batches that sit
+        in PINNED host memory (ResNet-18: 38.5 MB per step) take a detour that hides the PCIe transfer: the H2D copy goes
+        to one of two staging buffers on a copy stream — the host issues it while the GPU is still computing the previous
+        step — and the compute stream only does a device-to-device copy (microseconds) once the staged data has landed."""
+        for i, (dst, src) in enumerate(zip(shape.leaves, leaves)):
+            if not isinstance(dst, torch.Tensor):
+                continue
+            # the signature matched, so the shapes do: copy_ would otherwise broadcast a smaller batch silently
+            assert dst.shape == src.shape and dst.dtype == src.dtype, (key, i, dst.shape, src.shape)
+            staged = (isinstance(src, torch.Tensor) and not src.is_cuda and src.is_pinned()
+                      and src.numel() * src.element_size() >= self.STAGE_MIN_BYTES)
+            if not staged:
+                dst.copy_(src, non_blocking=True)
+                continue
+            if self._copy_stream is None:
+                self._copy_stream = torch.cuda.Stream(device=self.device)
+            slot = self._staging.get((key, i))
+            if slot is None:
+                slot = self._staging[key, i] = {'buf': [torch.empty_like(dst), torch.empty_like(dst)], 'next': 0,
+                                                'ready': [torch.cuda.Event(), torch.cuda.Event()],
+                                                'consumed': [torch.cuda.Event(), torch.cuda.Event()],
+                                                'used': [False, False]}
+            k = slot['next']
+            slot['next'] ^= 1
+            compute = torch.cuda.current_stream(self.device)
+            if slot['used'][k]:
+                self._copy_stream.wait_event(slot['consumed'][k])  # the step that last read this staging buffer has copied it out
+            with torch.cuda.stream(self._copy_stream):
+                slot['buf'][k].copy_(src, non_blocking=True)
+                slot['ready'][k].record(self._copy_stream)
+            compute.wait_event(slot['ready'][k])
+            dst.copy_(slot['buf'][k], non_blocking=True)
+            slot['consumed'][k].record(compute)
+            slot['used'][k] = True
+
+    def _static_inputs(self, shape, batch, leaves):
+        """The static inputs of `shape`'s graph, made on its first capture: device tensors like the batch's leaves, in the
+        batch's structure."""
+        if shape.leaves is None:
+            shape.leaves = [torch.empty_like(x, device=self.device) if isinstance(x, torch.Tensor) else x for x in leaves]
+            shape.batch = tree_unflatten(shape.leaves, tree_flatten(batch)[1])
+
+
+class GraphedTrainStep(_StaticBatchStep):
     def __init__(self, stage):
         self.stage = stage
         pipeline = stage.pipeline
@@ -194,11 +252,6 @@ class GraphedTrainStep:
     @property
     def static(self):
         return self.first.batch if self.first is not None else None
-
-    def _say(self, what, message):
-        if what not in self._said:
-            self._said.add(what)
-            self.stage.logger.warning(message)
 
     # ---- the fused step exchange -------------------------------------------------------------------------------------
     def _prepare_exchange(self, slab):
@@ -398,9 +451,7 @@ class GraphedTrainStep:
         shape = self.shapes.get(key)
         if shape is None:
             shape = self.shapes[key] = _ShapeGraph()
-        if shape.leaves is None:
-            shape.leaves = [torch.empty_like(x, device=self.device) if isinstance(x, torch.Tensor) else x for x in leaves]
-            shape.batch = tree_unflatten(shape.leaves, tree_flatten(batch)[1])
+        self._static_inputs(shape, batch, leaves)
         self._load(key, shape, leaves)
         if not self.bucket.attached():
             raise RuntimeError('cuda_graph mode: parameter .grad no longer alias the flat bucket')
@@ -528,44 +579,6 @@ class GraphedTrainStep:
         stream.wait_stream(side)
         return [a.elapsed_time(b) * 1e3 / per_graph for a, b in times]
 
-    STAGE_MIN_BYTES = 1 << 20
-
-    def _load(self, key, shape, leaves):
-        """Bring the batch's leaves into the static input buffers of its own signature's graph.  Large batches that sit
-        in PINNED host memory (ResNet-18: 38.5 MB per step) take a detour that hides the PCIe transfer: the H2D copy goes
-        to one of two staging buffers on a copy stream — the host issues it while the GPU is still computing the previous
-        step — and the compute stream only does a device-to-device copy (microseconds) once the staged data has landed."""
-        for i, (dst, src) in enumerate(zip(shape.leaves, leaves)):
-            if not isinstance(dst, torch.Tensor):
-                continue
-            # the signature matched, so the shapes do: copy_ would otherwise broadcast a smaller batch silently
-            assert dst.shape == src.shape and dst.dtype == src.dtype, (key, i, dst.shape, src.shape)
-            staged = (isinstance(src, torch.Tensor) and not src.is_cuda and src.is_pinned()
-                      and src.numel() * src.element_size() >= self.STAGE_MIN_BYTES)
-            if not staged:
-                dst.copy_(src, non_blocking=True)
-                continue
-            if self._copy_stream is None:
-                self._copy_stream = torch.cuda.Stream(device=self.device)
-            slot = self._staging.get((key, i))
-            if slot is None:
-                slot = self._staging[key, i] = {'buf': [torch.empty_like(dst), torch.empty_like(dst)], 'next': 0,
-                                                'ready': [torch.cuda.Event(), torch.cuda.Event()],
-                                                'consumed': [torch.cuda.Event(), torch.cuda.Event()],
-                                                'used': [False, False]}
-            k = slot['next']
-            slot['next'] ^= 1
-            compute = torch.cuda.current_stream(self.device)
-            if slot['used'][k]:
-                self._copy_stream.wait_event(slot['consumed'][k])  # the step that last read this staging buffer has copied it out
-            with torch.cuda.stream(self._copy_stream):
-                slot['buf'][k].copy_(src, non_blocking=True)
-                slot['ready'][k].record(self._copy_stream)
-            compute.wait_event(slot['ready'][k])
-            dst.copy_(slot['buf'][k], non_blocking=True)
-            slot['consumed'][k].record(compute)
-            slot['used'][k] = True
-
     def detach(self):
         """End of the stage: scalars still waiting for an exchange take the normal route; later stages see a plain slab.
         The graphs stay: the stage may train again."""
@@ -585,3 +598,164 @@ class GraphedTrainStep:
         if self._own_comm is not None:
             self._own_comm.close()
             self._own_comm = None
+
+
+class GraphedValStep(_StaticBatchStep):
+    """The validation step of TrainValStage.val_epoch as CUDA graphs (`TrainValStage.cuda_graph_val`).  One graph holds
+
+        slab.batching = True  ->  loss = stage.val_step(batch)  [user metrics are QUEUED, not launched]
+        ->  track_reduce(loss)  ->  _count_batch('val')  ->  ONE dmlb_metric_fold launch of slab.take_batch()
+
+    run under torch.no_grad(), so a replay is the user's forward plus one fold node, with no launch from Python.  A graph is
+    keyed by the batch signature (`batch_signature`) AND by the `training` flag of every module of every registered model,
+    snapshotted once per val epoch (`begin_epoch`): the stage never calls model.eval() itself, so a user who switches modes
+    in a hook (BatchNorm, dropout) gets a graph captured in that mode, never a replay of the other one.
+
+    Schedule: the first `cuda_graph_warmup` val steps (counted across epochs) run uncaptured; each key they meet counts as
+    seen.  After that, a key seen for the first time runs uncaptured, is captured on its next occurrence and replayed from
+    then on.  Keys beyond `cuda_graph_max_shapes`, and batches with an unhashable non-tensor leaf, always run uncaptured.
+    An uncaptured step is the same `_one_step` launched as it is: same kernels in the same order, so its results equal a
+    replay's bit for bit.
+
+    A val step issues no collective, so the ranks never have to pair up: each one replays, captures or runs uncaptured
+    as its own shard dictates, and ranks whose shards have different lengths meet again at the epoch-closing reduce.
+
+    Requirements, as for the captured training step: val_step must not synchronise with the host (no .item(), no printing
+    of tensors); python values it tracks are constants of the graph; the batch may influence it only through its
+    signature.  A metric must be tracked first in an uncaptured step — tracking a new metric inside a capture is refused."""
+
+    def __init__(self, stage):
+        self.stage = stage
+        self.device = stage.pipeline.device
+        if self.device is None or self.device.type != 'cuda':
+            raise RuntimeError('cuda_graph_val mode needs a CUDA device')
+        self.shapes = {}        # (batch signature, module modes) -> _ShapeGraph (graph None: seen once, or dropped)
+        self.modes = ()         # the module-mode snapshot of the current val epoch
+        self.loss = None        # the loss of the latest step, whichever kind it was
+        self.warmup_steps = 0
+        self.eager_steps = 0    # uncaptured steps, the warm-up ones included
+        self.replays = 0        # graph-driven steps, the real run after each capture included
+        self.captures = 0
+        self._pool = None
+        self._copy_stream = None
+        self._staging = {}
+        self._slab_generation = None
+        self._said = set()
+
+    def begin_epoch(self):
+        """Snapshot the `training` flag of every module of every registered model: part of every graph key this epoch."""
+        self.modes = tuple(m.training for model in self.stage.pipeline.models.values() for m in model.modules())
+
+    def _one_step(self, batch):
+        """One val step on `batch` (captured or run as it is): (loss, tensors the fold entries read)."""
+        stage = self.stage
+        slab = stage.tracker._slab_or_create()
+        slab.batching = True
+        try:
+            loss = stage.val_step(batch)
+            stage.track_reduce(stage.loss_metric_name(), loss)
+            stage._count_batch('val')
+            entries, keep = slab.take_batch()
+        finally:
+            slab.batching = False
+        for i in range(0, len(entries), N.MAX_FOLD_ENTRIES):
+            slab._launch_fold(entries[i:i + N.MAX_FOLD_ENTRIES])
+        return loss, keep
+
+    def __call__(self, batch):
+        key, leaves = batch_signature(batch)
+        if key is not None:
+            key = (key, self.modes)
+        slab = self.stage.tracker._slab_or_create()
+        if slab.generation != self._slab_generation:
+            self._invalidate(slab)
+        shape = self.shapes.get(key) if key is not None else None
+        warming = self.warmup_steps < self.stage.cuda_graph_warmup
+        if shape is not None and shape.graph is not None:
+            self._load(key, shape, leaves)
+            self._replay(shape)
+        elif shape is not None and not warming:
+            self._capture(key, batch, leaves)  # second occurrence, or again after the slab grew
+        else:
+            if warming:
+                self.warmup_steps += 1
+            if key is None:
+                self._say('unhashable', 'cuda_graph_val mode: a batch with an unhashable non-tensor leaf runs uncaptured')
+            elif shape is None and len(self.shapes) < self.stage.cuda_graph_max_shapes:
+                self.shapes[key] = _ShapeGraph()  # captured on its next occurrence
+            elif shape is None:
+                self._say('cap', f'cuda_graph_val mode: more than cuda_graph_max_shapes = '
+                                 f'{self.stage.cuda_graph_max_shapes} val batch shapes; further shapes run uncaptured')
+            with torch.no_grad():
+                self.loss, _ = self._one_step(batch)  # (the allocator is stream-ordered: the fold's inputs may go now)
+            self.eager_steps += 1
+        return self.loss
+
+    def _capture(self, key, batch, leaves):
+        shape = self.shapes[key]
+        self._static_inputs(shape, batch, leaves)
+        self._load(key, shape, leaves)
+        stream = torch.cuda.current_stream(self.device)
+        if stream == torch.cuda.default_stream(self.device):
+            raise RuntimeError('cuda_graph_val mode must not run on the legacy default stream (TrainingPipeline.run() '
+                               'puts the stages on its compute stream; do the same when driving a stage by hand)')
+        slab = self.stage.tracker._slab_or_create()
+        # host scalars queued by earlier steps (the train loop's misc/step_time_ms, scalars waiting in a captured training
+        # step's HostFeed) are launched NOW: inside the capture they would be baked into the graph and re-added by every
+        # replay.  Without the feed, the batch counters tracked inside the step become immediates of the graph's own fold
+        feed = slab.feed
+        slab.flush_all()
+        slab.feed = None
+        cells = slab.n_cells
+        # The val graphs share one memory pool of their own.  A capture may reuse memory another val capture freed (its
+        # intermediates), never memory another graph still holds (its loss, the tensors its fold entries read).  That is
+        # safe because the graphs replay one at a time on one stream and no graph's intermediates are read after another
+        # graph has replayed; the loss of a step is its own graph's output, which no other graph writes.  The training
+        # graphs' pool would be just as safe, but each class drops its pool when it drops its graphs; a pool of their own
+        # keeps the two lifetimes apart.  It costs the memory of one forward without saved activations.
+        if self._pool is None:
+            self._pool = torch.cuda.graph_pool_handle()
+        graph = torch.cuda.CUDAGraph()
+        before = N.launch_count()
+        try:
+            with torch.no_grad(), torch.cuda.graph(graph, pool=self._pool, stream=stream):
+                loss, keep = self._one_step(shape.batch)
+        finally:
+            slab.feed = feed
+        if slab.n_cells != cells:
+            # the new metric's cell reset was recorded, not run, and a replay would reset it every step
+            raise RuntimeError('cuda_graph_val mode: val_step tracked a metric for the first time while it was being '
+                               'captured; a batch signature must track the same metrics on every occurrence')
+        shape.kernels = N.launch_count() - before  # libdmlb kernels every replay re-runs
+        shape.graph, shape.loss, shape.keep = graph, loss, keep
+        self.captures += 1
+        self._slab_generation = slab.generation
+        self._replay(shape)  # capture only records: run the step once for real
+
+    def _replay(self, shape):
+        shape.graph.replay()
+        self.replays += 1
+        shape.replays += 1
+        self.loss = shape.loss
+
+    def _invalidate(self, slab):
+        """The metric slab was reallocated (it grew): every graph holds stale pointers.  Drop them all; each key is
+        captured again on its next occurrence."""
+        if any(s.graph is not None for s in self.shapes.values()):
+            torch.cuda.synchronize(self.device)
+            for s in self.shapes.values():
+                s.graph = s.loss = s.keep = None
+            self._pool = None
+        self._slab_generation = slab.generation
+
+    def detach(self):
+        """End of the stage.  A val step leaves nothing queued in the slab between steps, so there is nothing to hand
+        back; the graphs stay: the stage may validate again."""
+
+    def close(self):
+        """detach() and release every key's graph, static inputs and staging buffers."""
+        self.detach()
+        torch.cuda.synchronize(self.device)
+        self.shapes.clear()
+        self._staging.clear()
+        self._pool = None

@@ -116,9 +116,9 @@ class Stage:
         self.pipeline.barrier(self.barrier_timeout)
 
     def _post_stage(self):
-        graph = getattr(self, '_graph', None)
-        if graph is not None:
-            graph.detach()
+        for graph in (getattr(self, '_graph', None), getattr(self, '_val_graph', None)):
+            if graph is not None:
+                graph.detach()
         if getattr(self, '_gc_was_enabled', False):
             import gc
 
@@ -191,6 +191,14 @@ class TrainValStage(Stage):
         self.cuda_graph_max_shapes = 4
         self._graph = None
         self._eager_steps = 0
+        # Extension: replay the validation step from CUDA graphs too (graphstep.GraphedValStep): one graph per batch
+        # signature and mode of the models' modules holds val_step, the loss and batch-counter folds in ONE fold launch.
+        # Independent of `cuda_graph`: training may stay eager with any torch optimizer.  Uses cuda_graph_warmup and
+        # cuda_graph_max_shapes, counting its own warm-up steps and graphs.  Like the captured training step, val_step
+        # must not synchronise with the host, the python values it tracks are constants of the graph, and the batch may
+        # influence it only through its signature (shapes, dtypes, python values).
+        self.cuda_graph_val = False
+        self._val_graph = None
 
     # ---- lookups -----------------------------------------------------------------------------------------------------
     def _dataset(self, key):
@@ -342,9 +350,22 @@ class TrainValStage(Stage):
     def val_epoch(self):
         self.is_train = False
         self.metric_prefix = self.val_metric_prefix()
+        if self.cuda_graph_val:
+            self._graphed_val_epoch()
+            return
         for batch in self.val_dataset():
             self.track_reduce(self.loss_metric_name(), self.val_step(batch))
             self._count_batch('val')
+
+    def _graphed_val_epoch(self):
+        """Every batch through the captured val step: warm-up, uncaptured step, capture or replay, by its signature."""
+        if self._val_graph is None:
+            from .graphstep import GraphedValStep
+
+            self._val_graph = GraphedValStep(self)
+        self._val_graph.begin_epoch()
+        for batch in self.val_dataset():
+            self._val_graph(batch)
 
     def table_columns(self):
         loss = self.loss_metric_name()
