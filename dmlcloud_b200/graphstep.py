@@ -23,11 +23,14 @@ into ONE cudaGraph and replays it per batch.  What is different from the eager l
 
 Batches of several shapes — the short last batch of a loader without drop_last, dict batches, batches that carry python
 values — get one graph per batch signature (`batch_signature`: tree structure, (shape, dtype) of every tensor leaf, the
-value of every other leaf).  The first graph is captured on batch `cuda_graph_warmup + 1`.  After that, a signature seen
-for the first time runs `_one_step` UNCAPTURED (the "flat step": same code, same flat bucket, same fused exchange kernel;
-it also lets cuDNN / cuBLAS pick their algorithms for the new shape), is captured on its second occurrence and replayed
-from then on.  Signatures beyond `TrainValStage.cuda_graph_max_shapes`, and batches with an unhashable non-tensor leaf,
-always take the flat step.
+value of every other leaf).  This step and `GraphedValStep` follow one schedule (`_CapturedStep`): a key with a graph
+replays it; a key seen for the first time runs UNCAPTURED, is captured on its second sighting and replayed from then on;
+keys beyond `TrainValStage.cuda_graph_max_shapes`, and batches with an unhashable non-tensor leaf, always run uncaptured.
+The two differ in one rule only, the warm-up (`_due`).  Here the stage runs the `cuda_graph_warmup` eager steps before
+this step exists, and they are not sightings: the first graph is captured at once, on batch `cuda_graph_warmup + 1`.  The
+validation step runs its warm-up steps itself, uncaptured, and they count as sightings.  The uncaptured training step is
+the "flat step": same `_one_step`, same flat bucket, same fused exchange kernel; it also lets cuDNN / cuBLAS pick their
+algorithms for the new shape.
 
 Why the ranks stay paired whatever each one decides: every kind of training step — a replay of any signature's graph, a
 flat step, the real run that follows a capture — issues exactly ONE dmlb_comm_allreduce on the flat gradient bucket, with
@@ -43,6 +46,7 @@ signature (shapes, dtypes, python values), as any captured code must.
 `GraphedValStep` does the same for the validation step (`TrainValStage.cuda_graph_val`): val_step and its metric folds,
 one graph per batch signature and module-mode snapshot, no gradients, no optimizer, no collective.
 """
+import contextlib
 import ctypes
 
 import torch
@@ -103,25 +107,167 @@ def batch_signature(batch):
 
 
 class _ShapeGraph:
-    """What belongs to ONE batch signature: its static inputs, its graph and what the graph's nodes point at."""
+    """What belongs to ONE batch key: its static inputs, its graph and what the graph's nodes point at."""
 
     def __init__(self):
         self.leaves = None        # static inputs: device tensors (non-tensor leaves as the loader gave them)
-        self.batch = None         # the same leaves in the loader's structure: what train_step receives
-        self.graph = None
-        self.loss = None
+        self.batch = None         # the same leaves in the loader's structure: what the step receives
+        self.kernels = 0          # libdmlb kernels one replay re-runs
+        self.replays = 0
+        self.drop()
+
+    def drop(self):
+        """Forget the graph and what its nodes point at; the static inputs stay for the next capture."""
+        self.graph = self.loss = None
         self.step_metrics = None  # the dmlb_step_metrics descriptor baked into the graph (None: no live exchange)
         self.live_names = {}
         self.keep = None          # tensors the captured fold entries read: they must live as long as the graph
-        self.kernels = 0          # libdmlb kernels one replay re-runs
-        self.replays = 0
 
 
-class _StaticBatchStep:
-    """What the captured training and validation steps share: warnings said once, and the copy of a batch into the static
-    inputs of its signature's graph (`_load`).  Subclasses set `stage`, `device`, `_said`, `_copy_stream`, `_staging`."""
+@contextlib.contextmanager
+def _feed_detached(slab, feed):
+    """Launch every host scalar `slab` holds, queued or waiting in its feed ring, and keep python scalars off any feed
+    ring until the block ends; then `feed` receives them (None: they are queued for a launch of their own)."""
+    slab.flush_all()
+    slab.feed = None
+    try:
+        yield
+    finally:
+        slab.feed = feed
 
+
+class _CapturedStep:
+    """What the captured training and validation steps share: the table of batch keys (`shapes`), the schedule that
+    replays, captures or runs a batch uncaptured, the capture sequence, and the copy of a batch into the static inputs of
+    its key's graph (`_load`).
+
+    Schedule (`__call__`): a key that has a graph replays it.  Otherwise the subclass decides whether the key is due
+    (`_due`) and, if so, it is captured now.  Otherwise the batch runs uncaptured (`_uncaptured`) and a key seen for the
+    first time is registered, to be captured on a later sighting.  Keys beyond `cuda_graph_max_shapes`, and batches with
+    an unhashable non-tensor leaf (key None), always run uncaptured.  When the metric slab is reallocated every graph is
+    dropped; each key is captured again on its next sighting.
+
+    A capture (`_capture`) records the subclass's `_record(shape)` on the very stream the uncaptured steps ran on, with
+    the host scalars queued so far launched first, then runs the graph once for real.  Each captured step keeps one memory
+    pool for its graphs.  A capture may reuse memory another capture freed (its intermediates), never memory another
+    graph still holds (its loss, the tensors its fold entries read).  That is safe because the graphs replay one at a time
+    on one stream and no graph's intermediates are read after another graph has replayed; the loss of a step is its own
+    graph's output, which no other graph writes.  The training and validation graphs could share one pool just as safely,
+    but each step drops its pool when it drops its graphs; a pool of its own keeps the two lifetimes apart.  It costs the
+    validation step the memory of one forward without saved activations.
+
+    A subclass names its stage option (`MODE`) and supplies `_due`, `_record` and `_uncaptured`; it may add to the key
+    (`_signature`) and to the set-up before every step (`_before_step`) and before a capture (`_before_capture`)."""
+
+    MODE = None  # the stage option that turns the step on, for messages
     STAGE_MIN_BYTES = 1 << 20
+
+    def __init__(self, stage):
+        self.stage = stage
+        self.device = stage.pipeline.device
+        if self.device is None or self.device.type != 'cuda':
+            raise RuntimeError(f'{self.MODE} mode needs a CUDA device')
+        self.shapes = {}   # key -> _ShapeGraph (graph None: seen once, or dropped when the slab grew)
+        self.loss = None   # the loss of the latest step, whichever kind it was
+        self.replays = 0   # graph-driven steps of every key, the real run after each capture included
+        self.captures = 0
+        self._pool = None
+        self._slab_generation = None
+        self._copy_stream = None  # side stream + double-buffered staging for large pinned host batches (see _load)
+        self._staging = {}
+        self._said = set()
+
+    _signature = staticmethod(batch_signature)  # (key, leaves) of a batch
+
+    def _before_step(self):
+        """Runs before every step, whatever its kind."""
+
+    def __call__(self, batch):
+        key, leaves = self._signature(batch)
+        slab = self.stage.tracker._slab_or_create()
+        if slab.generation != self._slab_generation:
+            self._invalidate(slab)
+        self._before_step()
+        shape = self.shapes.get(key) if key is not None else None
+        if shape is not None and shape.graph is not None:
+            self._load(key, shape, leaves)
+            self._replay(shape)
+        elif self._due(key, shape):
+            self._capture(key, batch, leaves)
+        else:
+            if key is None:
+                self._say('unhashable', f'{self.MODE} mode: a batch with an unhashable non-tensor leaf runs uncaptured')
+            elif shape is None and len(self.shapes) < self.stage.cuda_graph_max_shapes:
+                self.shapes[key] = _ShapeGraph()  # captured on a later sighting
+            elif shape is None:
+                self._say('cap', f'{self.MODE} mode: more than cuda_graph_max_shapes = '
+                                 f'{self.stage.cuda_graph_max_shapes} batch shapes; further shapes run uncaptured')
+            self._uncaptured(batch)
+        return self.loss
+
+    def _before_capture(self, slab):
+        """Set-up before a capture; returns the feed ring that receives python scalars once the capture is done."""
+        return slab.feed
+
+    def _capture(self, key, batch, leaves):
+        shape = self.shapes.get(key)
+        if shape is None:
+            shape = self.shapes[key] = _ShapeGraph()
+        self._static_inputs(shape, batch, leaves)
+        self._load(key, shape, leaves)
+        stream = torch.cuda.current_stream(self.device)
+        if stream == torch.cuda.default_stream(self.device):
+            raise RuntimeError(f'{self.MODE} mode must not run on the legacy default stream (TrainingPipeline.run() puts '
+                               'the stages on its compute stream; do the same when driving a stage by hand)')
+        slab = self.stage.tracker._slab_or_create()
+        # host scalars queued by earlier steps (the train loop's misc/step_time_ms, scalars waiting in a captured training
+        # step's HostFeed) are launched NOW: inside the capture they would be baked into the graph and re-added by every
+        # replay.  Without a feed, the scalars tracked inside the step become immediates of the graph's own fold
+        with _feed_detached(slab, self._before_capture(slab)):
+            if self._pool is None:
+                self._pool = torch.cuda.graph_pool_handle()
+            graph = torch.cuda.CUDAGraph()
+            before = N.launch_count()
+            # capture on the very stream the uncaptured steps ran on: autograd's AccumulateGrad nodes (stashed by DDP at
+            # construction) then already live on the capturing stream and no cross-stream edge enters the graph
+            with torch.cuda.graph(graph, pool=self._pool, stream=stream):
+                self._record(shape)
+            shape.kernels = N.launch_count() - before  # libdmlb kernels every replay re-runs
+        shape.graph = graph
+        self.captures += 1
+        self._slab_generation = slab.generation
+        self._replay(shape)  # capture only records: run the step once for real
+        return shape
+
+    def _replay(self, shape):
+        exchange = shape.step_metrics is not None  # a training graph with the fused step exchange
+        if exchange:
+            self._before_exchange()
+        shape.graph.replay()
+        self.replays += 1
+        shape.replays += 1
+        self.loss = shape.loss
+        if exchange:
+            self._after_exchange(shape.live_names)
+
+    def _invalidate(self, slab):
+        """The metric slab was reallocated (it grew): every graph holds stale pointers.  Drop them all; each key is
+        captured again on its next sighting, without a second warm-up.  True if there were graphs to drop."""
+        self._slab_generation = slab.generation
+        if not any(s.graph is not None for s in self.shapes.values()):
+            return False
+        torch.cuda.synchronize(self.device)
+        for s in self.shapes.values():
+            s.drop()
+        self._pool = None
+        return True
+
+    def close(self):
+        """Release every key's graph, static inputs and staging buffers."""
+        torch.cuda.synchronize(self.device)
+        self.shapes.clear()
+        self._staging.clear()
+        self._pool = None
 
     def _say(self, what, message):
         if what not in self._said:
@@ -172,13 +318,12 @@ class _StaticBatchStep:
             shape.batch = tree_unflatten(shape.leaves, tree_flatten(batch)[1])
 
 
-class GraphedTrainStep(_StaticBatchStep):
+class GraphedTrainStep(_CapturedStep):
+    MODE = 'cuda_graph'
+
     def __init__(self, stage):
-        self.stage = stage
+        super().__init__(stage)
         pipeline = stage.pipeline
-        self.device = pipeline.device
-        if self.device.type != 'cuda':
-            raise RuntimeError('cuda_graph mode needs a CUDA device')
         self.lib = N.cuda_lib(self.device.index)
         self.world = dist.get_world_size()
         self.models = list(pipeline.models.values())
@@ -219,12 +364,8 @@ class GraphedTrainStep(_StaticBatchStep):
                                'gradient set that fits grad_arena_bytes')
         self.comm = comm
         self.sumsq = torch.zeros(1, dtype=torch.float64, device=self.device)
-        self.shapes = {}   # batch signature -> _ShapeGraph (graph None: seen once, or dropped when the slab grew)
-        self.first = None  # the first captured signature: `graph`, `step_metrics` and `kernels_in_graph` describe it
-        self.loss = None   # the loss of the latest step, whichever kind it was
-        self.replays = 0   # graph-driven steps of every signature, the real run after each capture included
+        self.first = None  # the first captured signature: `step_metrics` and `kernels_in_graph` describe it
         self.flat_steps = 0
-        self.captures = 0
         self.exchanges = 0  # fused step exchanges with a metric descriptor == the device counter's value
         self.kernels_in_graph = 0
         # fused step exchange state, shared by every signature and by the flat step (created once, before the first step)
@@ -235,23 +376,10 @@ class GraphedTrainStep(_StaticBatchStep):
         self.live_names = {}
         self.zero_in_optimizer = False
         self._feed_fixed = False  # the feed's column map is assigned: every graph and flat step uses that same map
-        self._pool = None
-        self._copy_stream = None  # side stream + double-buffered staging for large pinned host batches (see _load)
-        self._staging = {}
-        self._slab_generation = None
-        self._said = set()
-
-    @property
-    def graph(self):
-        return self.first.graph if self.first is not None else None
 
     @property
     def step_metrics(self):
         return self.first.step_metrics if self.first is not None else None
-
-    @property
-    def static(self):
-        return self.first.batch if self.first is not None else None
 
     # ---- the fused step exchange -------------------------------------------------------------------------------------
     def _prepare_exchange(self, slab):
@@ -409,62 +537,21 @@ class GraphedTrainStep(_StaticBatchStep):
         self._optimize()
         return loss, metrics, live_names, keep
 
-    # ---- the three kinds of step -------------------------------------------------------------------------------------
-    def __call__(self, batch):
-        key, leaves = batch_signature(batch)
-        slab = self.stage.tracker._slab_or_create()
-        if slab.generation != self._slab_generation:
-            self._invalidate(slab)
-        self._sync_lr()
-        shape = self.shapes.get(key) if key is not None else None
-        if shape is not None and shape.graph is not None:
-            self._load(key, shape, leaves)
-            self._replay(shape)
-        elif shape is not None or (key is not None and self.first is None):
-            self._capture(key, batch, leaves)  # second occurrence, first graph of all, or again after the slab grew
-        else:
-            if key is None:
-                self._say('unhashable', 'cuda_graph mode: a batch with an unhashable non-tensor leaf runs uncaptured')
-            elif len(self.shapes) < self.stage.cuda_graph_max_shapes:
-                self.shapes[key] = _ShapeGraph()  # captured on its next occurrence
-            else:
-                self._say('cap', f'cuda_graph mode: more than cuda_graph_max_shapes = {self.stage.cuda_graph_max_shapes} '
-                                 'batch shapes; further shapes run uncaptured')
-            self._flat_step(batch)
-        return self.loss
+    # ---- the schedule and the three kinds of step ----------------------------------------------------------------------
+    def _due(self, key, shape):
+        """A key is captured on its second sighting; the first graph of all at once, since the stage's eager warm-up
+        steps ran before this step existed and are not sightings."""
+        return shape is not None or (key is not None and self.first is None)
 
-    def capture(self, batch):
-        """Capture the step for `batch`'s signature on `batch` (its values are consumed: this is a real training step)."""
-        key, leaves = batch_signature(batch)
-        if key is None:
-            raise RuntimeError('cuda_graph mode: a batch with an unhashable non-tensor leaf cannot be captured')
-        self._sync_lr()
-        return self._capture(key, batch, leaves)
-
-    def _sync_lr(self):
+    def _before_step(self):
         for opt in self.stage.optimizers():
             sync_lr = getattr(opt, 'sync_device_lr', None)
             if sync_lr is not None:
                 sync_lr()  # a scheduler changed group['lr']: one tiny fill, only when the value actually changed
 
-    def _capture(self, key, batch, leaves):
-        shape = self.shapes.get(key)
-        if shape is None:
-            shape = self.shapes[key] = _ShapeGraph()
-        self._static_inputs(shape, batch, leaves)
-        self._load(key, shape, leaves)
+    def _before_capture(self, slab):
         if not self.bucket.attached():
             raise RuntimeError('cuda_graph mode: parameter .grad no longer alias the flat bucket')
-        stream = torch.cuda.current_stream(self.device)
-        if stream == torch.cuda.default_stream(self.device):
-            raise RuntimeError('cuda_graph mode must not run on the legacy default stream (TrainingPipeline.run() puts '
-                               'the stages on its compute stream; do the same when driving a stage by hand)')
-        stage = self.stage
-        slab = stage.tracker._slab_or_create()
-        # host scalars queued by the last eager step must be launched NOW: inside the capture they would be baked into
-        # the graph and re-added by every replay
-        slab.flush_all()  # (also hands scalars still waiting in the feed ring to a normal fold launch)
-        slab.feed = None
         self._prepare_exchange(slab)
         if self.first is None:
             # DDP rebuilds its buckets in the first forward after the first backward, with a host-to-device copy that
@@ -472,11 +559,9 @@ class GraphedTrainStep(_StaticBatchStep):
             # capture their first graph at the same step; afterwards the call returns at once)
             for m in self.ddp_models:
                 m.reducer._rebuild_buckets()
-        torch.cuda.synchronize(self.device)
-        if self.first is None:
             # `optimizer.zero_grad()` of the next step (reference stage.py:300) is fused into the K5 / K6 launch when ONE
             # flat optimizer owns every gradient of the bucket: one kernel node and one pass over the gradients fewer
-            opts = list(stage.optimizers())
+            opts = list(self.stage.optimizers())
             self.zero_in_optimizer = (len(opts) == 1 and getattr(opts[0], 'device_lr', False)
                                       and len(opts[0].param_groups) == 1
                                       and opts[0]._flat_grad_base(opts[0].param_groups[0], opts[0]._flat[0]) ==
@@ -484,21 +569,14 @@ class GraphedTrainStep(_StaticBatchStep):
             if self.zero_in_optimizer:
                 opts[0].zero_grad_in_step = True
                 self.bucket.flat.zero_()  # once, outside the graph: every replay and flat step leaves zeros behind
-        # All graphs share one memory pool.  A capture may reuse memory another capture freed (its intermediates), never
-        # memory another graph still holds (its loss, the tensors its fold entries read).  That is safe because the graphs
-        # replay one at a time on one stream and no graph's intermediates are read after another graph has replayed;
-        # the loss of a step is its own graph's output, which no other graph writes.
-        if self._pool is None:
-            self._pool = torch.cuda.graph_pool_handle()
-        graph = torch.cuda.CUDAGraph()
-        # capture on the very stream the warm-up steps ran on: autograd's AccumulateGrad nodes (stashed by DDP at
-        # construction) then already live on the capturing stream and no cross-stream edge enters the graph
-        before = N.launch_count()
-        with torch.cuda.graph(graph, pool=self._pool, stream=stream):
-            loss, metrics, live_names, keep = self._one_step(shape.batch, eager=False)
-        shape.kernels = N.launch_count() - before  # libdmlb kernels every replay re-runs
-        shape.graph, shape.loss, shape.step_metrics, shape.live_names, shape.keep = graph, loss, metrics, live_names, keep
-        self.captures += 1
+        torch.cuda.synchronize(self.device)
+        return self.feed  # from now on python scalars of the feed's cells wait for the next exchange
+
+    def _record(self, shape):
+        shape.loss, shape.step_metrics, shape.live_names, shape.keep = self._one_step(shape.batch, eager=False)
+
+    def _capture(self, key, batch, leaves):
+        shape = super()._capture(key, batch, leaves)
         if self.first is None:
             self.first = shape
         if shape is self.first:
@@ -506,53 +584,29 @@ class GraphedTrainStep(_StaticBatchStep):
         elif shape.kernels != self.first.kernels:
             self._say(('kernels', key), f'cuda_graph mode: the graph of batch signature {key} re-runs {shape.kernels} '
                                         f'libdmlb kernels per replay, the first graph {self.first.kernels}')
-        self._slab_generation = slab.generation
-        slab.feed = self.feed  # from now on python scalars of the feed's cells wait for the next exchange
-        self._replay(shape)  # capture only records: run the step once for real
-        return self.loss
+        return shape
 
-    def _replay(self, shape):
-        exchange = shape.step_metrics is not None
-        if exchange:
-            self._before_exchange()
-        shape.graph.replay()
-        self.replays += 1
-        shape.replays += 1
-        self.loss = shape.loss
-        if exchange:
-            self._after_exchange(shape.live_names)
-
-    def _flat_step(self, batch):
-        """The step of a signature without a graph, run as it is: the same `_one_step` on the same flat bucket and the
-        same single fused exchange as a replay, so the ranks' collectives stay paired."""
+    def _uncaptured(self, batch):
+        """The flat step: the step of a signature without a graph, run as it is — the same `_one_step` on the same flat
+        bucket and the same single fused exchange as a replay, so the ranks' collectives stay paired."""
         leaves, spec = tree_flatten(batch)
         batch = tree_unflatten([x.to(self.device, non_blocking=True) if isinstance(x, torch.Tensor) else x
                                 for x in leaves], spec)
         slab = self.stage.tracker._slab_or_create()
         self._prepare_exchange(slab)
+        # a step that assigns the feed's column map hands the scalars tracked so far to the normal route.  (The allocator
+        # is stream-ordered: the fold entries' tensors may go once the step is launched.)
         assign = self.feed is not None and not self._feed_fixed
-        if assign:  # the feed's column map is assigned by this step: scalars tracked so far take the normal route
-            slab.flush_all()
-            slab.feed = None
-        loss, metrics, live_names, _ = self._one_step(batch, eager=True)  # (the allocator is stream-ordered: the fold
-        if assign:                                                        # entries' tensors may go once it is launched)
-            slab.feed = self.feed
+        with _feed_detached(slab, self.feed) if assign else contextlib.nullcontext():
+            loss, metrics, live_names, _ = self._one_step(batch, eager=True)
         self.flat_steps += 1
         self.loss = loss
         if metrics is not None:
             self._after_exchange(live_names)
 
     def _invalidate(self, slab):
-        """The metric slab was reallocated (it grew): every graph holds stale pointers.  Drop them all; each signature is
-        captured again on its next occurrence, without a second warm-up."""
-        if any(s.graph is not None for s in self.shapes.values()):
-            torch.cuda.synchronize(self.device)
-            for s in self.shapes.values():
-                s.graph = s.loss = s.step_metrics = s.keep = None
-                s.live_names = {}
-            self._pool = None
+        if super()._invalidate(slab):
             self._feed_fixed = False  # no graph holds the column map any more: the next step assigns it afresh
-        self._slab_generation = slab.generation
 
     def time_gradient_sync(self, reps=20, per_graph=20):
         """Device time (us) of ONE gradient-sync launch on the flat bucket (without the metric CTA): `per_graph` of them
@@ -584,23 +638,20 @@ class GraphedTrainStep(_StaticBatchStep):
         The graphs stay: the stage may train again."""
         slab = self.stage.tracker._slab
         if slab is not None and slab.feed is not None and slab.feed is self.feed:
-            slab.flush_all()
-            slab.feed = None
+            with _feed_detached(slab, None):
+                pass
 
     def close(self):
-        """detach() and release every signature's graph, static inputs and staging buffers."""
+        """detach(), release every signature's graph, static inputs and staging buffers, and the step's own communicator."""
         self.detach()
-        torch.cuda.synchronize(self.device)
-        self.shapes.clear()
-        self._staging.clear()
+        super().close()
         self.first = None
-        self._pool = None
         if self._own_comm is not None:
             self._own_comm.close()
             self._own_comm = None
 
 
-class GraphedValStep(_StaticBatchStep):
+class GraphedValStep(_CapturedStep):
     """The validation step of TrainValStage.val_epoch as CUDA graphs (`TrainValStage.cuda_graph_val`).  One graph holds
 
         slab.batching = True  ->  loss = stage.val_step(batch)  [user metrics are QUEUED, not launched]
@@ -611,11 +662,9 @@ class GraphedValStep(_StaticBatchStep):
     snapshotted once per val epoch (`begin_epoch`): the stage never calls model.eval() itself, so a user who switches modes
     in a hook (BatchNorm, dropout) gets a graph captured in that mode, never a replay of the other one.
 
-    Schedule: the first `cuda_graph_warmup` val steps (counted across epochs) run uncaptured; each key they meet counts as
-    seen.  After that, a key seen for the first time runs uncaptured, is captured on its next occurrence and replayed from
-    then on.  Keys beyond `cuda_graph_max_shapes`, and batches with an unhashable non-tensor leaf, always run uncaptured.
-    An uncaptured step is the same `_one_step` launched as it is: same kernels in the same order, so its results equal a
-    replay's bit for bit.
+    Schedule: the captured steps' one schedule (`_CapturedStep`).  The warm-up runs here: the first `cuda_graph_warmup`
+    val steps (counted across epochs) run uncaptured, and each key they meet counts as seen.  An uncaptured step is the
+    same `_one_step` launched as it is: same kernels in the same order, so its results equal a replay's bit for bit.
 
     A val step issues no collective, so the ranks never have to pair up: each one replays, captures or runs uncaptured
     as its own shard dictates, and ranks whose shards have different lengths meet again at the epoch-closing reduce.
@@ -624,28 +673,23 @@ class GraphedValStep(_StaticBatchStep):
     of tensors); python values it tracks are constants of the graph; the batch may influence it only through its
     signature.  A metric must be tracked first in an uncaptured step — tracking a new metric inside a capture is refused."""
 
+    MODE = 'cuda_graph_val'
+
     def __init__(self, stage):
-        self.stage = stage
-        self.device = stage.pipeline.device
-        if self.device is None or self.device.type != 'cuda':
-            raise RuntimeError('cuda_graph_val mode needs a CUDA device')
-        self.shapes = {}        # (batch signature, module modes) -> _ShapeGraph (graph None: seen once, or dropped)
+        super().__init__(stage)
         self.modes = ()         # the module-mode snapshot of the current val epoch
-        self.loss = None        # the loss of the latest step, whichever kind it was
         self.warmup_steps = 0
         self.eager_steps = 0    # uncaptured steps, the warm-up ones included
-        self.replays = 0        # graph-driven steps, the real run after each capture included
-        self.captures = 0
-        self._pool = None
-        self._copy_stream = None
-        self._staging = {}
-        self._slab_generation = None
-        self._said = set()
 
     def begin_epoch(self):
         """Snapshot the `training` flag of every module of every registered model: part of every graph key this epoch."""
         self.modes = tuple(m.training for model in self.stage.pipeline.models.values() for m in model.modules())
 
+    def _signature(self, batch):
+        key, leaves = batch_signature(batch)
+        return ((key, self.modes) if key is not None else None), leaves
+
+    @torch.no_grad()
     def _one_step(self, batch):
         """One val step on `batch` (captured or run as it is): (loss, tensors the fold entries read)."""
         stage = self.stage
@@ -662,100 +706,23 @@ class GraphedValStep(_StaticBatchStep):
             slab._launch_fold(entries[i:i + N.MAX_FOLD_ENTRIES])
         return loss, keep
 
-    def __call__(self, batch):
-        key, leaves = batch_signature(batch)
-        if key is not None:
-            key = (key, self.modes)
-        slab = self.stage.tracker._slab_or_create()
-        if slab.generation != self._slab_generation:
-            self._invalidate(slab)
-        shape = self.shapes.get(key) if key is not None else None
-        warming = self.warmup_steps < self.stage.cuda_graph_warmup
-        if shape is not None and shape.graph is not None:
-            self._load(key, shape, leaves)
-            self._replay(shape)
-        elif shape is not None and not warming:
-            self._capture(key, batch, leaves)  # second occurrence, or again after the slab grew
-        else:
-            if warming:
-                self.warmup_steps += 1
-            if key is None:
-                self._say('unhashable', 'cuda_graph_val mode: a batch with an unhashable non-tensor leaf runs uncaptured')
-            elif shape is None and len(self.shapes) < self.stage.cuda_graph_max_shapes:
-                self.shapes[key] = _ShapeGraph()  # captured on its next occurrence
-            elif shape is None:
-                self._say('cap', f'cuda_graph_val mode: more than cuda_graph_max_shapes = '
-                                 f'{self.stage.cuda_graph_max_shapes} val batch shapes; further shapes run uncaptured')
-            with torch.no_grad():
-                self.loss, _ = self._one_step(batch)  # (the allocator is stream-ordered: the fold's inputs may go now)
-            self.eager_steps += 1
-        return self.loss
+    def _due(self, key, shape):
+        """A key is captured on its second sighting; the warm-up steps are sightings too, an unhashable batch among them
+        counting toward the warm-up."""
+        if self.warmup_steps < self.stage.cuda_graph_warmup:
+            self.warmup_steps += 1
+            return False
+        return shape is not None
 
-    def _capture(self, key, batch, leaves):
-        shape = self.shapes[key]
-        self._static_inputs(shape, batch, leaves)
-        self._load(key, shape, leaves)
-        stream = torch.cuda.current_stream(self.device)
-        if stream == torch.cuda.default_stream(self.device):
-            raise RuntimeError('cuda_graph_val mode must not run on the legacy default stream (TrainingPipeline.run() '
-                               'puts the stages on its compute stream; do the same when driving a stage by hand)')
+    def _record(self, shape):
         slab = self.stage.tracker._slab_or_create()
-        # host scalars queued by earlier steps (the train loop's misc/step_time_ms, scalars waiting in a captured training
-        # step's HostFeed) are launched NOW: inside the capture they would be baked into the graph and re-added by every
-        # replay.  Without the feed, the batch counters tracked inside the step become immediates of the graph's own fold
-        feed = slab.feed
-        slab.flush_all()
-        slab.feed = None
         cells = slab.n_cells
-        # The val graphs share one memory pool of their own.  A capture may reuse memory another val capture freed (its
-        # intermediates), never memory another graph still holds (its loss, the tensors its fold entries read).  That is
-        # safe because the graphs replay one at a time on one stream and no graph's intermediates are read after another
-        # graph has replayed; the loss of a step is its own graph's output, which no other graph writes.  The training
-        # graphs' pool would be just as safe, but each class drops its pool when it drops its graphs; a pool of their own
-        # keeps the two lifetimes apart.  It costs the memory of one forward without saved activations.
-        if self._pool is None:
-            self._pool = torch.cuda.graph_pool_handle()
-        graph = torch.cuda.CUDAGraph()
-        before = N.launch_count()
-        try:
-            with torch.no_grad(), torch.cuda.graph(graph, pool=self._pool, stream=stream):
-                loss, keep = self._one_step(shape.batch)
-        finally:
-            slab.feed = feed
+        shape.loss, shape.keep = self._one_step(shape.batch)
         if slab.n_cells != cells:
             # the new metric's cell reset was recorded, not run, and a replay would reset it every step
             raise RuntimeError('cuda_graph_val mode: val_step tracked a metric for the first time while it was being '
                                'captured; a batch signature must track the same metrics on every occurrence')
-        shape.kernels = N.launch_count() - before  # libdmlb kernels every replay re-runs
-        shape.graph, shape.loss, shape.keep = graph, loss, keep
-        self.captures += 1
-        self._slab_generation = slab.generation
-        self._replay(shape)  # capture only records: run the step once for real
 
-    def _replay(self, shape):
-        shape.graph.replay()
-        self.replays += 1
-        shape.replays += 1
-        self.loss = shape.loss
-
-    def _invalidate(self, slab):
-        """The metric slab was reallocated (it grew): every graph holds stale pointers.  Drop them all; each key is
-        captured again on its next occurrence."""
-        if any(s.graph is not None for s in self.shapes.values()):
-            torch.cuda.synchronize(self.device)
-            for s in self.shapes.values():
-                s.graph = s.loss = s.keep = None
-            self._pool = None
-        self._slab_generation = slab.generation
-
-    def detach(self):
-        """End of the stage.  A val step leaves nothing queued in the slab between steps, so there is nothing to hand
-        back; the graphs stay: the stage may validate again."""
-
-    def close(self):
-        """detach() and release every key's graph, static inputs and staging buffers."""
-        self.detach()
-        torch.cuda.synchronize(self.device)
-        self.shapes.clear()
-        self._staging.clear()
-        self._pool = None
+    def _uncaptured(self, batch):
+        self.loss, _ = self._one_step(batch)  # (the allocator is stream-ordered: the fold's inputs may go now)
+        self.eager_steps += 1

@@ -116,9 +116,6 @@ class Stage:
         self.pipeline.barrier(self.barrier_timeout)
 
     def _post_stage(self):
-        for graph in (getattr(self, '_graph', None), getattr(self, '_val_graph', None)):
-            if graph is not None:
-                graph.detach()
         if getattr(self, '_gc_was_enabled', False):
             import gc
 
@@ -199,6 +196,11 @@ class TrainValStage(Stage):
         # influence it only through its signature (shapes, dtypes, python values).
         self.cuda_graph_val = False
         self._val_graph = None
+
+    def _post_stage(self):
+        if self._graph is not None:
+            self._graph.detach()  # (a captured val step leaves nothing queued in the slab between steps)
+        super()._post_stage()
 
     # ---- lookups -----------------------------------------------------------------------------------------------------
     def _dataset(self, key):

@@ -40,7 +40,8 @@ def run(drop_last, per_step):
     from dmlcloud_b200.util.data import DeviceShardedDataset
 
     times = {'flat': [], 'capture': [], 'replay': []}
-    saved = {}
+    step_cls = graphstep.GraphedTrainStep
+    saved = {}  # name -> the step class's own function (None: inherited from the base class)
     if per_step:
         def timed(kind, fn):
             def wrapper(self, *a, **k):
@@ -52,11 +53,11 @@ def run(drop_last, per_step):
                 return out
             return wrapper
 
-        for kind, name in (('flat', '_flat_step'), ('capture', '_capture')):
-            saved[name] = getattr(graphstep.GraphedTrainStep, name)
-            setattr(graphstep.GraphedTrainStep, name, timed(kind, saved[name]))
-        call = graphstep.GraphedTrainStep.__call__
-        saved['__call__'] = call
+        for kind, name in (('flat', '_uncaptured'), ('capture', '_capture')):
+            saved[name] = vars(step_cls).get(name)
+            setattr(step_cls, name, timed(kind, getattr(step_cls, name)))
+        call = step_cls.__call__
+        saved['__call__'] = vars(step_cls).get('__call__')
 
         def call_timed(self, batch):  # a replay is a call that neither captured nor ran uncaptured
             n = (self.flat_steps, self.captures, self.replays)
@@ -68,7 +69,7 @@ def run(drop_last, per_step):
                 times['replay'].append((time.perf_counter() - t0) * 1e3)
             return out
 
-        graphstep.GraphedTrainStep.__call__ = call_timed
+        step_cls.__call__ = call_timed
 
     g = torch.Generator().manual_seed(0)
     images = torch.randint(0, 256, (N_IMAGES, 1, 28, 28), dtype=torch.uint8, generator=g)
@@ -120,7 +121,10 @@ def run(drop_last, per_step):
             p.run()
     finally:
         for name, fn in saved.items():
-            setattr(graphstep.GraphedTrainStep, name, fn)
+            if fn is None:
+                delattr(step_cls, name)
+            else:
+                setattr(step_cls, name, fn)
     gs = stage._graph
     steps = len(p.datasets['train'])
     out = {'drop_last': drop_last, 'steps_per_epoch': steps, 'epoch_ms': stage.epoch_ms,
