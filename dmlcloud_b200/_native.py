@@ -130,6 +130,9 @@ SIGNATURES = {
     'dmlb_image_batch_u8': (c_int, [c_void_p, c_void_p, c_int64, c_int32, c_int32, c_int32, c_int32, c_int32, c_int32,
                                     c_int, c_int, c_uint64, c_int64, POINTER(ImageNorm), c_void_p, c_int, c_int,
                                     c_void_p, c_void_p]),
+    'dmlb_image_resample_u8': (c_int, [c_void_p, c_void_p, c_void_p, c_int64, c_int32, c_int32, c_int32, c_int32, c_int32,
+                                       c_int32, c_int32, c_int32, c_int32, POINTER(ImageNorm), c_void_p, c_int, c_int,
+                                       c_void_p]),
 }
 
 _lib = None

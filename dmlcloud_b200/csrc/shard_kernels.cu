@@ -6,6 +6,8 @@
 // (bit-exact host computation — the same numpy MT19937 stream the reference uses) and each step is one gather kernel:
 //   out[i, :] = (float(images[idx[i], :]) / 255 - mean) / std                      784 B read, 3136 (fp32) B written / sample
 // HBM-bound byte work: 16 pixels (one 128-bit load) per thread, 4x 128-bit stores, rows found through idx[] (L2-resident).
+#include <cmath>
+
 #include "dmlb_common.cuh"
 
 namespace dmlb {
@@ -150,9 +152,10 @@ struct ImageBand {
 };
 
 // Walks a contiguous run of output elements in memory order: NCHW runs stay in one channel plane, NHWC runs step c fastest.
-template <bool kVecLoad, bool kNHWC>
+// Band: any band type with members C, ow and value(r, x, c) (ImageBand, ResampleBand).
+template <class Band, bool kNHWC>
 struct ImageCursor {
-    const ImageBand<kVecLoad> &b;
+    const Band &b;
     int r, x, c;
     __device__ __forceinline__ uint32_t next() {
         const uint32_t v = b.value(r, x, c);
@@ -259,13 +262,13 @@ __global__ void __launch_bounds__(kImageThreads) image_batch_u8_kernel(const Ima
             const int C = a.C, ow = a.ow;
             image_store_run<kBf16>(a.out, i * plane * C + (long long)y0 * ow * C, nr * ow * C, [&](int k) {
                 const int p = k / C;
-                return ImageCursor<kVecLoad, true>{band, p / ow, p - (p / ow) * ow, k - p * C};
+                return ImageCursor<ImageBand<kVecLoad>, true>{band, p / ow, p - (p / ow) * ow, k - p * C};
             });
         } else {
             for (int c = 0; c < a.C; ++c) {
                 const int ow = a.ow;
                 image_store_run<kBf16>(a.out, (i * a.C + c) * plane + (long long)y0 * ow, nr * ow, [&](int k) {
-                    return ImageCursor<kVecLoad, false>{band, k / ow, k - (k / ow) * ow, c};
+                    return ImageCursor<ImageBand<kVecLoad>, false>{band, k / ow, k - (k / ow) * ow, c};
                 });
             }
         }
@@ -278,6 +281,222 @@ static void launch_image(bool vec_load, int grid, size_t smem, cudaStream_t st, 
         image_batch_u8_kernel<kBf16, kNHWC, true><<<grid, kImageThreads, smem, st>>>(a);
     else
         image_batch_u8_kernel<kBf16, kNHWC, false><<<grid, kImageThreads, smem, st>>>(a);
+}
+
+
+// ---- resampled colour images: box -> antialiased bilinear resize -> window -> flip -> normalise ---------------------
+// (dmlb_image_resample_u8; include/dmlb.h states the rule.)  One CTA job = one band of up to `rows` output rows of one
+// sample.  The CTA builds the sample's column taps (xmin, xsize, weights) for the window's columns and the row taps of
+// the band, runs the horizontal pass over the band's source rows into an fp32 [srows][out_w * C] tile in shared memory,
+// then the vertical pass, written in the output's contiguous order by image_store_run.  Source bytes are read through
+// L1 (a box row's bytes are read by neighbouring columns' taps) and mapped through a 256-entry fl32(byte) / 255 table.
+// Every operation of the tap and pixel arithmetic is rounded once, as written (no FMA contraction).
+
+constexpr int kResampleThreads = 256;
+constexpr int kResampleMaxScale = 8;          // H <= 8 resize_h, W <= 8 resize_w: at most 2 * 8 + 1 taps per output
+constexpr int kResampleMaxRowElems = 1024;    // out_w * C
+constexpr int kResampleMaxSide = 32768;       // H, W, resize_h, resize_w: tap positions stay exact in fp32
+constexpr int kResampleBandBytes = 32768;     // target size of a band's tile + row taps (one row may need up to 76 KB)
+constexpr int kResampleCtasPerSm = 4;
+
+struct ResampleArgs {
+    const uint8_t *images;
+    const long long *idx;
+    const int *boxes;
+    void *out;
+    long long batch, sample_bytes;
+    int H, W, C, rh, rw, win_top, win_left, oh, ow;
+    int rows, bands, srows, kx, ky;  // band height, bands per sample, tile rows, column / row tap stride
+    float mean[4], std[4];
+};
+
+// One axis of one sample: ATen's antialiased bilinear filter (aten/src/ATen/native/cpu/UpSampleKernel.cpp,
+// _compute_indices_min_size_weights_aa with align_corners = false), with its C++ types: scale, support, center and the
+// weights are fp32; center, the bounds and the filter argument are formed in fp64 where C++ promotes, then rounded.
+struct ResampleAxis {
+    float scale, support, invscale;
+    int K, n_in;
+
+    __device__ __forceinline__ ResampleAxis(int in, int out) : n_in(in) {
+        scale = __fdiv_rn((float)in, (float)out);
+        support = scale >= 1.0f ? scale : 1.0f;
+        invscale = scale >= 1.0f ? (float)(1.0 / (double)scale) : 1.0f;
+        K = (int)ceilf(support) * 2 + 1;
+    }
+    __device__ __forceinline__ float center(int i) const { return (float)((double)scale * ((double)i + 0.5)); }
+    __device__ __forceinline__ int xmin(int i) const {
+        return max((int)((double)__fsub_rn(center(i), support) + 0.5), 0);
+    }
+    __device__ __forceinline__ int xend(int i) const {  // one past the last tap before the clamp to K
+        return min((int)((double)__fadd_rn(center(i), support) + 0.5), n_in);
+    }
+    // xmin and xsize of output index i; weights w[0, xsize), normalised by their fp32 sum taken in increasing j.
+    __device__ __forceinline__ void taps(int i, int &x0, int &n, float *w) const {
+        const float c = center(i);
+        x0 = xmin(i);
+        n = min(max(xend(i) - x0, 0), K);
+        float total = 0.0f;
+        for (int j = 0; j < n; ++j) {
+            const float t = __fsub_rn((float)(j + x0), c);
+            const float arg = fabsf((float)(((double)t + 0.5) * (double)invscale));
+            w[j] = arg < 1.0f ? __fsub_rn(1.0f, arg) : 0.0f;
+            total = __fadd_rn(total, w[j]);
+        }
+        if (total != 0.0f)
+            for (int j = 0; j < n; ++j) w[j] = __fdiv_rn(w[j], total);
+    }
+};
+
+// One band of one resampled sample: the fp32 tile holds the horizontal pass of source rows [ylo, ylo + srows) of the
+// box; value() runs the vertical pass of window pixel (r, x, c) of the band and normalises it.
+template <bool kBf16>
+struct ResampleBand {
+    const float *tile, *wy, *mean, *std;
+    const int *ymin, *ysize;
+    int ylo, rowf, ky, C, ow, flip, ok;
+
+    __device__ __forceinline__ uint32_t value(int r, int x, int c) const {
+        if (!ok) return kBf16 ? 0x7fc0u : 0x7fc00000u;  // a box outside the image: quiet NaN, nothing read
+        const int u = flip ? ow - 1 - x : x;
+        const float *col = tile + (ymin[r] - ylo) * rowf + u * C + c;
+        const float *w = wy + r * ky;
+        const int n = ysize[r];
+        float acc = __fmul_rn(col[0], w[0]);
+        for (int j = 1; j < n; ++j) acc = __fadd_rn(acc, __fmul_rn(col[j * rowf], w[j]));
+        const float v = __fdiv_rn(__fsub_rn(acc, mean[c]), std[c]);
+        return kBf16 ? (uint32_t)f32_to_bf16(v) : __float_as_uint(v);
+    }
+};
+
+// Dynamic shared memory of one CTA, in this order (every piece a multiple of 4 bytes).
+struct ResampleSmem {
+    float *tile, *wx, *wy;
+    int *xmin, *xsize, *ymin, *ysize;
+
+    __host__ __device__ static size_t bytes(int srows, int rowf, int ow, int kx, int rows, int ky) {
+        return 4 * ((size_t)srows * rowf + (size_t)ow * (kx + 2) + (size_t)rows * (ky + 2));
+    }
+    __device__ ResampleSmem(float *base, const ResampleArgs &a) {
+        tile = base;
+        wx = tile + (size_t)a.srows * a.ow * a.C;
+        wy = wx + (size_t)a.ow * a.kx;
+        xmin = reinterpret_cast<int *>(wy + (size_t)a.rows * a.ky);
+        xsize = xmin + a.ow;
+        ymin = xsize + a.ow;
+        ysize = ymin + a.rows;
+    }
+};
+
+template <bool kBf16, bool kNHWC>
+__global__ void __launch_bounds__(kResampleThreads) image_resample_u8_kernel(const ResampleArgs a) {
+    extern __shared__ float s_dyn[];
+    __shared__ float s_lut[256];
+    __shared__ float s_norm[8];
+    const ResampleSmem sm(s_dyn, a);
+    for (int e = threadIdx.x; e < 256; e += blockDim.x) s_lut[e] = __fdiv_rn((float)e, 255.0f);
+    if (threadIdx.x < 4) {
+        s_norm[threadIdx.x] = a.mean[threadIdx.x];
+        s_norm[4 + threadIdx.x] = a.std[threadIdx.x];
+    }
+    const long long jobs = a.batch * a.bands;
+    const int rowf = a.ow * a.C, plane = a.oh * a.ow;
+    for (long long job = blockIdx.x; job < jobs; job += gridDim.x) {
+        const long long i = job / a.bands;
+        const int y0 = (int)(job - i * a.bands) * a.rows;
+        const int nr = min(a.rows, a.oh - y0);
+        const int *box = a.boxes + 5 * i;
+        const int top = box[0], left = box[1], bh = box[2], bw = box[3], flip = box[4] != 0;
+        const int ok = top >= 0 && left >= 0 && bh >= 1 && bw >= 1 && top <= a.H - bh && left <= a.W - bw;
+        const ResampleAxis ax(ok ? bw : 1, a.rw), ay(ok ? bh : 1, a.rh);
+        const int ylo = ay.xmin(a.win_top + y0);
+        const int nsrc = ok ? min(ay.xend(a.win_top + y0 + nr - 1) - ylo, a.srows) : 0;
+        __syncthreads();  // the previous job's readers are done with the tile and the taps (and the tables are built)
+        if (ok) {
+            for (int u = threadIdx.x; u < a.ow; u += blockDim.x)
+                ax.taps(a.win_left + u, sm.xmin[u], sm.xsize[u], sm.wx + u * a.kx);
+            for (int r = threadIdx.x; r < nr; r += blockDim.x)
+                ay.taps(a.win_top + y0 + r, sm.ymin[r], sm.ysize[r], sm.wy + r * a.ky);
+        }
+        __syncthreads();
+        const uint8_t *img = a.images + a.idx[i] * a.sample_bytes + ((long long)(top + ylo) * a.W + left) * a.C;
+        for (int t = threadIdx.x; t < nsrc * rowf; t += blockDim.x) {
+            const int sr = t / rowf, e = t - sr * rowf, u = e / a.C, c = e - u * a.C;
+            const uint8_t *src = img + ((long long)sr * a.W + sm.xmin[u]) * a.C + c;
+            const float *w = sm.wx + u * a.kx;
+            const int n = sm.xsize[u];
+            float acc = __fmul_rn(s_lut[__ldg(src)], w[0]);
+            for (int j = 1; j < n; ++j) acc = __fadd_rn(acc, __fmul_rn(s_lut[__ldg(src + j * a.C)], w[j]));
+            sm.tile[t] = acc;
+        }
+        __syncthreads();
+        const ResampleBand<kBf16> band{sm.tile, sm.wy, s_norm, s_norm + 4, sm.ymin, sm.ysize, ylo, rowf, a.ky, a.C,
+                                       a.ow, flip, ok};
+        if (kNHWC) {
+            const int C = a.C, ow = a.ow;
+            image_store_run<kBf16>(a.out, i * plane * C + (long long)y0 * ow * C, nr * ow * C, [&](int k) {
+                const int p = k / C;
+                return ImageCursor<ResampleBand<kBf16>, true>{band, p / ow, p - (p / ow) * ow, k - p * C};
+            });
+        } else {
+            for (int c = 0; c < a.C; ++c) {
+                const int ow = a.ow;
+                image_store_run<kBf16>(a.out, (i * a.C + c) * plane + (long long)y0 * ow, nr * ow, [&](int k) {
+                    return ImageCursor<ResampleBand<kBf16>, false>{band, k / ow, k - (k / ow) * ow, c};
+                });
+            }
+        }
+    }
+}
+
+// Band geometry of one launch (host): taps per output on each axis at the largest box the image allows, the band
+// height whose tile and row taps fit kResampleBandBytes (at least one row), and the tile rows that band can need.
+// The column taps take ow (kx + 2) words whatever the band height, so a launch needs at most the column taps plus the
+// larger of kResampleBandBytes and a band of one row: kResampleMaxSmem at the widest row and the largest downscale.
+struct ResamplePlan {
+    int kx, ky, rows, bands, srows;
+    size_t smem;
+};
+
+static int resample_taps(int in, int out) {
+    const float scale = (float)in / (float)out;
+    return (int)std::ceil(scale >= 1.0f ? scale : 1.0f) * 2 + 1;
+}
+
+// Source rows a band of `rows` output rows can read: (rows - 1) scale + 2 support + 1, plus 2 for rounding.
+static int resample_srows(int rows, int H, int rh) {
+    const double scale = (double)H / (double)rh, support = scale >= 1.0 ? scale : 1.0;
+    const int n = (int)std::floor((rows - 1) * scale + 2.0 * support + 1.0) + 2;
+    return n < H ? n : H;
+}
+
+constexpr int kResampleMaxTaps = 2 * kResampleMaxScale + 1;
+constexpr int kResampleMaxSrows = 2 * kResampleMaxScale + 3;  // resample_srows(1, H, rh) at H = 8 rh
+constexpr size_t kResampleMaxSmem = 4 * ((size_t)kResampleMaxRowElems * (kResampleMaxTaps + 2) +
+                                         (size_t)kResampleMaxSrows * kResampleMaxRowElems + (kResampleMaxTaps + 2));
+static_assert(kResampleMaxSmem > (size_t)kResampleBandBytes, "a band of one row at the limits exceeds the band target");
+static_assert(kResampleMaxSmem + 2048 <= 227 * 1024, "every accepted launch must fit the opt-in shared memory of sm_90");
+
+static ResamplePlan resample_plan(int H, int W, int C, int rh, int rw, int oh, int ow) {
+    ResamplePlan p;
+    p.kx = resample_taps(W, rw);
+    p.ky = resample_taps(H, rh);
+    const size_t row_bytes = (size_t)ow * C * 4;
+    auto band_bytes = [&](int rows) { return 4 * (size_t)rows * (p.ky + 2) + resample_srows(rows, H, rh) * row_bytes; };
+    int rows = 1;
+    while (rows < oh && band_bytes(rows + 1) <= (size_t)kResampleBandBytes) ++rows;
+    p.bands = (oh + rows - 1) / rows;
+    p.rows = (oh + p.bands - 1) / p.bands;
+    p.srows = resample_srows(p.rows, H, rh);
+    p.smem = ResampleSmem::bytes(p.srows, ow * C, ow, p.kx, p.rows, p.ky);
+    return p;
+}
+
+template <bool kBf16, bool kNHWC>
+static int launch_resample(int grid, size_t smem, cudaStream_t st, const ResampleArgs &a) {
+    DMLB_CUDA(cudaFuncSetAttribute(image_resample_u8_kernel<kBf16, kNHWC>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                   (int)smem));
+    image_resample_u8_kernel<kBf16, kNHWC><<<grid, kResampleThreads, smem, st>>>(a);
+    return launched();
 }
 
 }  // namespace dmlb
@@ -379,6 +598,50 @@ int dmlb_image_batch_u8(const uint8_t *images, const int64_t *idx, int64_t batch
             launch_image<false, false>(vec_load, grid, smem, st, a);
     }
     return launched();
+}
+
+
+int dmlb_image_resample_u8(const uint8_t *images, const int64_t *idx, const int32_t *boxes, int64_t batch, int32_t H,
+                           int32_t W, int32_t C, int32_t resize_h, int32_t resize_w, int32_t win_top, int32_t win_left,
+                           int32_t out_h, int32_t out_w, const dmlb_image_norm *norm, void *out, int out_bf16,
+                           int channels_last, void *stream) {
+    if (batch < 0 || !norm || C < 1 || C > 4) return DMLB_EINVAL;
+    for (int32_t side : {H, W, resize_h, resize_w, out_h, out_w})
+        if (side < 1 || side > kResampleMaxSide) return DMLB_EINVAL;
+    if ((long long)H > (long long)kResampleMaxScale * resize_h || (long long)W > (long long)kResampleMaxScale * resize_w)
+        return DMLB_EINVAL;
+    if (win_top < 0 || win_left < 0 || win_top > resize_h - out_h || win_left > resize_w - out_w) return DMLB_EINVAL;
+    if ((long long)out_w * C > kResampleMaxRowElems) return DMLB_EINVAL;
+    for (int c = 0; c < C; ++c)
+        if (norm->std[c] == 0.0f) return DMLB_EINVAL;
+    if (batch > 0 && (!images || !idx || !boxes || !out)) return DMLB_EINVAL;
+    if (((uintptr_t)out & (out_bf16 ? 1 : 3)) != 0 || ((uintptr_t)boxes & 3) != 0) return DMLB_EALIGN;
+    if (batch == 0) return DMLB_OK;
+
+    const ResamplePlan p = resample_plan(H, W, C, resize_h, resize_w, out_h, out_w);
+    ResampleArgs a;
+    a.images = images;
+    a.idx = (const long long *)idx;
+    a.boxes = boxes;
+    a.out = out;
+    a.batch = batch;
+    a.sample_bytes = (long long)H * W * C;
+    a.H = H, a.W = W, a.C = C, a.rh = resize_h, a.rw = resize_w, a.win_top = win_top, a.win_left = win_left;
+    a.oh = out_h, a.ow = out_w;
+    a.rows = p.rows, a.bands = p.bands, a.srows = p.srows, a.kx = p.kx, a.ky = p.ky;
+    for (int c = 0; c < 4; ++c) {
+        a.mean[c] = c < C ? norm->mean[c] : 0.0f;
+        a.std[c] = c < C ? norm->std[c] : 1.0f;
+    }
+    const long long jobs = batch * p.bands;
+    const long long cap = (long long)sm_count() * kResampleCtasPerSm;
+    const int grid = (int)(jobs < cap ? jobs : cap);
+    cudaStream_t st = (cudaStream_t)stream;
+    if (out_bf16)
+        return channels_last ? launch_resample<true, true>(grid, p.smem, st, a)
+                             : launch_resample<true, false>(grid, p.smem, st, a);
+    return channels_last ? launch_resample<false, true>(grid, p.smem, st, a)
+                         : launch_resample<false, false>(grid, p.smem, st, a);
 }
 
 }  // extern "C"

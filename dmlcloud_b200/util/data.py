@@ -13,7 +13,8 @@ batches through instead of falling into the general path.
 New (SURVEY §8f-1): `DeviceShardedDataset` keeps the whole uint8 dataset in HBM and produces each batch with one
 gather + normalise kernel (libdmlb dmlb_shard_gather_u8) instead of a host DataLoader + H2D copy per step.
 `DeviceImageDataset` does the same for colour images (HWC uint8) with pad / random or centre crop / horizontal flip /
-per-channel normalisation in one kernel (dmlb_image_batch_u8).
+per-channel normalisation in one kernel (dmlb_image_batch_u8), and `DeviceResizedImageDataset` does the ImageNet
+recipes (RandomResizedCrop or Resize + CenterCrop, flip, normalise) with one resampling kernel (dmlb_image_resample_u8).
 """
 from concurrent.futures import ThreadPoolExecutor
 from typing import Iterable, Sequence
@@ -233,15 +234,18 @@ class DeviceShardedDataset:
         n = self.shard_len()
         return n // self.batch_size if self.drop_last else -(-n // self.batch_size)
 
-    def epoch_indices(self):
-        """This rank's indices for the current epoch, on the device (and the host list for inspection)."""
-        n = self.images.shape[0]
-        N = self._N
-        lib = N.cuda_lib(self.device.index)
-        order = np.arange(n)
+    def _epoch_order(self):
+        """The epoch's permutation of all N indices on the host; this rank's shard is order[rank::world][:shard_len()]."""
+        order = np.arange(self.images.shape[0])
         if self.shuffle:
             np.random.Generator(np.random.MT19937(self.seed + self.epoch)).shuffle(order)
-        perm = torch.from_numpy(order).to(self.device, non_blocking=False)
+        return order
+
+    def epoch_indices(self):
+        """This rank's indices for the current epoch, on the device (and the host list for inspection)."""
+        N = self._N
+        lib = N.cuda_lib(self.device.index)
+        perm = torch.from_numpy(self._epoch_order()).to(self.device, non_blocking=False)
         count = self.shard_len()
         idx = torch.empty(count, dtype=torch.int64, device=self.device)
         N.check(lib.dmlb_shard_slice(perm.data_ptr(), 0, count, self.rank, self.world_size, idx.data_ptr(),
@@ -351,6 +355,163 @@ class DeviceImageDataset(DeviceShardedDataset):
             y = torch.empty(b, dtype=torch.int64, device=self.device)
             view = idx[start:start + b]
             self._launch(view, x)
+            N.check(lib.dmlb_shard_gather_i64(self.labels.data_ptr(), view.data_ptr(), b, y.data_ptr(), N.stream_ptr()),
+                    'shard_gather_i64')
+            yield x, y
+
+
+_GAMMA = np.uint64(0x9E3779B97F4A7C15)
+
+
+def _mix(z):
+    """SplitMix64's finaliser on uint64 arrays (the hash of dmlb_image_batch_u8, include/dmlb.h)."""
+    with np.errstate(over='ignore'):
+        z = (z ^ (z >> np.uint64(30))) * np.uint64(0xBF58476D1CE4E5B9)
+        z = (z ^ (z >> np.uint64(27))) * np.uint64(0x94D049BB133111EB)
+    return z ^ (z >> np.uint64(31))
+
+
+def resized_crop_boxes(rows, H, W, scale, ratio, seed, epoch, hflip):
+    """int32 [len(rows), 5] {top, left, height, width, flipped}: torchvision RandomResizedCrop.get_params for every
+    row, its uniform draws taken from the counter hash h = mix(mix(mix(seed + g) ^ (epoch + g)) ^ (row + g)), so a box
+    depends only on (seed, epoch, row).  Attempt a (0..9) takes the area fraction from the 53-bit uniform of
+    mix(h + (2 + 3a) g), the log aspect ratio from mix(h + (3 + 3a) g) and the offsets from mix(h + (4 + 3a) g) (top from
+    its low, left from its high 32 bits, u32 * n >> 32); w and h round halves to even; after 10 failed attempts the box
+    is torchvision's central fallback.  flipped = mix(h + g) >> 63 when hflip.  fp64 numpy, vectorised over the rows."""
+    rows = np.asarray(rows, dtype=np.int64)
+    with np.errstate(over='ignore'):
+        h = _mix(np.uint64(seed % (1 << 64)) + _GAMMA)
+        h = _mix(h ^ (np.uint64(epoch % (1 << 64)) + _GAMMA))
+        h = _mix(h ^ (rows.astype(np.uint64) + _GAMMA))
+
+        def word(k, sel=slice(None)):
+            return _mix(h[sel] + np.uint64(k) * _GAMMA)
+
+        def u53(k):
+            return (word(k) >> np.uint64(11)).astype(np.float64) * 2.0 ** -53
+
+        def below(u32, n):
+            return ((u32 * n.astype(np.uint64)) >> np.uint64(32)).astype(np.int64)
+
+        in_ratio = W / H
+        if in_ratio < min(ratio):
+            fw, fh = W, int(round(W / min(ratio)))
+        elif in_ratio > max(ratio):
+            fh, fw = H, int(round(H * max(ratio)))
+        else:
+            fw, fh = W, H
+        box = np.tile(np.asarray([(H - fh) // 2, (W - fw) // 2, fh, fw], dtype=np.int64), (len(rows), 1))
+        done = np.zeros(len(rows), dtype=bool)
+        lr0, lr1 = np.log(ratio[0]), np.log(ratio[1])
+        for a in range(10):
+            target = H * W * (scale[0] + (scale[1] - scale[0]) * u53(2 + 3 * a))
+            aspect = np.exp(lr0 + (lr1 - lr0) * u53(3 + 3 * a))
+            w = np.rint(np.sqrt(target * aspect)).astype(np.int64)
+            hh = np.rint(np.sqrt(target / aspect)).astype(np.int64)
+            ok = ~done & (w > 0) & (w <= W) & (hh > 0) & (hh <= H)
+            if ok.any():
+                off = word(4 + 3 * a, ok)
+                box[ok] = np.stack([below(off & np.uint64(0xFFFFFFFF), H - hh[ok] + 1),
+                                    below(off >> np.uint64(32), W - w[ok] + 1), hh[ok], w[ok]], axis=-1)
+                done |= ok
+        flip = (_mix(h + _GAMMA) >> np.uint64(63)).astype(np.int64) if hflip else np.zeros(len(rows), dtype=np.int64)
+    return np.concatenate([box, flip[:, None]], axis=1).astype(np.int32)
+
+
+class DeviceResizedImageDataset(DeviceImageDataset):
+    """Device-resident colour-image dataset with the ImageNet recipes (SURVEY §8f-1), one resampling launch per batch
+    (dmlb_image_resample_u8) plus the label gather.
+
+    images: uint8 [N, H, W, C] (HWC, C <= 4), labels: int64 [N].  size: int or (h, w) of the output.
+      random=True  (training): torchvision RandomResizedCrop(size, scale, ratio) -> RandomHorizontalFlip (if hflip)
+                   -> Normalize; the boxes of an epoch are sampled on the host (resized_crop_boxes) and uploaded once.
+      random=False (validation): Resize(resize) -> CenterCrop(size) -> Normalize (flipped when hflip, like training).
+    Resampling is antialiased bilinear (torchvision's default), as include/dmlb.h states.  x is [B, C, h, w] in
+    `memory_format`, in `out_dtype`.  A sample's box and flip depend only on (aug_seed, epoch, its dataset index), so
+    they are the same at every rank and world size.  Sharding, shuffle, even_shards and drop_last are
+    DeviceShardedDataset's.  The kernel takes image and resized sides of at most 32768, resizes at
+    most 8x down on each axis and writes rows of at most 1024 values; the constructor refuses anything else.
+    """
+
+    def __init__(self, images, labels, batch_size, mean, std, size, scale=(0.08, 1.0), ratio=(3 / 4, 4 / 3),
+                 random=True, resize=None, hflip=False, memory_format=torch.contiguous_format,
+                 out_dtype=torch.float32, shuffle=True, even_shards=True, seed=0, aug_seed=None, rank=None,
+                 world_size=None, device=None, drop_last=False):
+        super().__init__(images, labels, batch_size, mean, std, crop=None, padding=0, random_crop=random, hflip=hflip,
+                         memory_format=memory_format, out_dtype=out_dtype, shuffle=shuffle, even_shards=even_shards,
+                         seed=seed, aug_seed=aug_seed, rank=rank, world_size=world_size, device=device,
+                         drop_last=drop_last)
+        H, W, C = self.item_shape
+        size = (int(size), int(size)) if isinstance(size, (int, np.integer)) else tuple(int(v) for v in size)
+        if len(size) != 2 or min(size) < 1:
+            raise ValueError(f'size must be a positive int or (h, w), got {size}')
+        self.crop = size
+        self.scale, self.ratio = tuple(float(v) for v in scale), tuple(float(v) for v in ratio)
+        if random:
+            if not 0.0 < self.scale[0] <= self.scale[1] <= 1.0:
+                raise ValueError(f'scale must satisfy 0 < scale[0] <= scale[1] <= 1, got {self.scale}')
+            if not 0.0 < self.ratio[0] <= self.ratio[1]:
+                raise ValueError(f'ratio must satisfy 0 < ratio[0] <= ratio[1], got {self.ratio}')
+            if resize is not None:
+                raise ValueError('resize is for validation (random=False); training resizes every box to size')
+            self.resized, self.window = size, (0, 0)
+        else:
+            if resize is None or int(resize) < 1:
+                raise ValueError('validation (random=False) needs resize, the short side S of Resize(S)')
+            short, long = min(H, W), max(H, W)
+            S, L = int(resize), int(int(resize) * long / short)
+            self.resized = (L, S) if W <= H else (S, L)
+            if size[0] > self.resized[0] or size[1] > self.resized[1]:
+                raise ValueError(f'size {size} is larger than the resized image {self.resized}')
+            self.window = tuple(int(round((r - s) / 2.0)) for r, s in zip(self.resized, size))
+        if max(H, W, *self.resized) > 32768:
+            raise ValueError(f'{H}x{W} images resized to {self.resized}: the kernel takes sides of at most 32768')
+        if H > 8 * self.resized[0] or W > 8 * self.resized[1]:
+            raise ValueError(f'{H}x{W} images resized to {self.resized} is more than an 8x downscale')
+        if size[1] * C > 1024:
+            raise ValueError(f'size[1] * C = {size[1] * C} is above the 1024 values per output row the kernel takes')
+
+    def epoch_boxes(self):
+        """int32 [shard_len(), 5] numpy {top, left, height, width, flipped} of this rank's samples this epoch, in
+        iteration order."""
+        H, W, _ = self.item_shape
+        rows = self._epoch_order()[self.rank::self.world_size][:self.shard_len()]
+        if self.random_crop:
+            return resized_crop_boxes(rows, H, W, self.scale, self.ratio, self.aug_seed, self.epoch, self.hflip)
+        boxes = np.tile(np.asarray([0, 0, H, W, 0], dtype=np.int32), (len(rows), 1))
+        if self.hflip:
+            boxes[:, 4] = resized_crop_boxes(rows, H, W, self.scale, self.ratio, self.aug_seed, self.epoch, True)[:, 4]
+        return boxes
+
+    def _launch(self, idx, x, boxes):
+        N = self._N
+        H, W, C = self.item_shape
+        lib = N.cuda_lib(self.device.index)
+        N.check(lib.dmlb_image_resample_u8(self.images.data_ptr(), idx.data_ptr(), boxes.data_ptr(), idx.numel(), H, W,
+                                           C, self.resized[0], self.resized[1], self.window[0], self.window[1],
+                                           self.crop[0], self.crop[1], self._norm, x.data_ptr(),
+                                           int(self.out_dtype == torch.bfloat16),
+                                           int(self.memory_format == torch.channels_last), N.stream_ptr()),
+                'image_resample_u8')
+
+    def augment_params(self):
+        """(indices, boxes): this rank's dataset indices for the current epoch in iteration order, and the device int32
+        [count, 5] {top, left, height, width, flipped} the batches of this epoch use."""
+        return self.epoch_indices(), torch.from_numpy(self.epoch_boxes()).to(self.device)
+
+    def __iter__(self):
+        N = self._N
+        lib = N.cuda_lib(self.device.index)
+        idx, boxes = self.augment_params()
+        count = idx.numel()
+        for start in range(0, count, self.batch_size):
+            b = min(self.batch_size, count - start)
+            if b < self.batch_size and self.drop_last:
+                return
+            x = self._empty(b)
+            y = torch.empty(b, dtype=torch.int64, device=self.device)
+            view = idx[start:start + b]
+            self._launch(view, x, boxes[start:start + b])
             N.check(lib.dmlb_shard_gather_i64(self.labels.data_ptr(), view.data_ptr(), b, y.data_ptr(), N.stream_ptr()),
                     'shard_gather_i64')
             yield x, y

@@ -393,6 +393,37 @@ int dmlb_image_batch_u8(const uint8_t *images, const int64_t *idx, int64_t batch
                         const dmlb_image_norm *norm, void *out, int out_bf16, int channels_last, int32_t *params_out,
                         void *stream);
 
+/* Resampled colour-image batch: gather + box + antialiased bilinear resize + window + horizontal flip + per-channel
+ * normalise, one launch.  torchvision RandomResizedCrop (box per sample, resize = out, window at 0) and
+ * Resize(S) + CenterCrop (box = the whole image, window centred) are two settings of it.
+ *   images : uint8 [n, H, W, C] (HWC), C in 1..4; row i of the batch is images[idx[i]]
+ *   boxes  : DEVICE int32 [batch][5] {top, left, height, width, flipped} of every sample, in source pixels
+ *   out    : logical [batch, C, out_h, out_w], NCHW (channels_last == 0) or NHWC in memory, fp32 or bf16 (RNE)
+ * Sample i: the box of its image is resized to resize_h x resize_w, the window of out_h x out_w at (win_top, win_left)
+ * of the result is taken and mirrored horizontally when flipped != 0 (resize first, then flip, as torchvision).
+ * Resize = ATen's antialiased bilinear filter (interpolate(mode='bilinear', antialias=True, align_corners=False)),
+ * one axis of in -> out samples, per output index o, with ATen's types (f32 = fp32, f64 = fp64, one rounding each):
+ *   scale = f32(in) / f32(out); support = scale >= 1 ? scale : 1; K = 2 ceil(support) + 1
+ *   invscale = scale >= 1 ? f32(1.0 / f64(scale)) : 1;   center = f32(f64(scale) * (o + 0.5))
+ *   xmin = max(trunc(f64(center - support) + 0.5), 0);  xsize = clamp(min(trunc(f64(center + support) + 0.5), in) - xmin, 0, K)
+ *   w_j = max(0, 1 - |f32((f64(f32(j + xmin) - center) + 0.5) * invscale)|) for j < xsize, each divided by their fp32
+ *         sum taken in increasing j
+ * Pixels: v = f32(byte) / 255; the horizontal pass into fp32, then the vertical pass, each out = v_0 w_0 + v_1 w_1 + ...
+ * in increasing j with one rounding per multiply and per add (no FMA); then out = (v - mean[c]) / std[c].
+ * Accepted range (anything else: DMLB_EINVAL, nothing launched): C in 1..4; H, W, resize_h, resize_w, out_h, out_w in
+ * 1..32768; H <= 8 resize_h and W <= 8 resize_w (downscale at most 8x on each axis, at most 17 taps per output); the
+ * window inside the resized image; out_w * C <= 1024; std[c] != 0 for c < C; non-NULL norm, and images / idx / boxes /
+ * out when batch > 0.  DMLB_EALIGN: out not aligned to its element or boxes not to 4 bytes.  Every accepted argument
+ * set launches: a launch needs at most 156 KB of shared memory (the column taps of the widest row plus a band of one
+ * row at 8x downscale; taller bands keep their tile and row taps within 32 KB).  Boxes live in device memory and are
+ * not checked by the host: a box that is not inside the image (top, left >= 0, height, width >= 1, top + height <= H,
+ * left + width <= W) reads nothing and writes quiet NaN over its sample.  Any images alignment works.
+ * Algorithmic bytes/sample: box bytes read (at most) + out_h * out_w * C * (4 | 2) written + 20 B of box. */
+int dmlb_image_resample_u8(const uint8_t *images, const int64_t *idx, const int32_t *boxes, int64_t batch, int32_t H,
+                           int32_t W, int32_t C, int32_t resize_h, int32_t resize_w, int32_t win_top, int32_t win_left,
+                           int32_t out_h, int32_t out_w, const dmlb_image_norm *norm, void *out, int out_bf16,
+                           int channels_last, void *stream);
+
 #ifdef __cplusplus
 }
 #endif
