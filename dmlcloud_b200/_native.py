@@ -133,6 +133,9 @@ SIGNATURES = {
     'dmlb_image_resample_u8': (c_int, [c_void_p, c_void_p, c_void_p, c_int64, c_int32, c_int32, c_int32, c_int32, c_int32,
                                        c_int32, c_int32, c_int32, c_int32, POINTER(ImageNorm), c_void_p, c_int, c_int,
                                        c_void_p]),
+    'dmlb_image_mix': (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, POINTER(c_float), c_int64, c_int32, c_int32,
+                               c_int32, c_int, c_double, c_int32, c_int32, c_int32, c_int32, c_int32, c_void_p, c_int,
+                               c_int, c_void_p, c_void_p]),
 }
 
 _lib = None

@@ -499,6 +499,181 @@ static int launch_resample(int grid, size_t smem, cudaStream_t st, const Resampl
     return launched();
 }
 
+// ---- batch mixing: random erasing -> MixUp or CutMix -> soft targets (dmlb_image_mix) --------------------------------
+// (include/dmlb.h states the rule.)  Thread t owns V consecutive elements of a sample (one 16-byte output store: 4 fp32
+// or 8 bf16 values; V = 1 when a sample's elements or the pointers are not 16-byte aligned) and walks a segment of the
+// batch in order, keeping the previous sample's erased values in registers: the fp32 scratch batch is read once, plus
+// the partner of each segment's first sample, and `out` is written once.  The segments of one position are spread over
+// blockIdx.y so that a small batch still fills the GPU.  The targets are written by the same threads afterwards.
+
+constexpr int kMixThreads = 256;
+constexpr int kMixUnroll = 4;       // samples loaded ahead of their stores
+constexpr int kMixCtasPerSm = 8;    // target grid: enough segments to put this many CTAs on every SM
+constexpr int kMixMaxSide = 32768;  // h, w
+
+struct MixArgs {
+    const float *src;
+    const long long *idx, *labels;
+    const int *erase;
+    void *out, *targets;
+    long long batch, S;        // samples, elements per sample
+    long long nvec;            // positions per sample (S / V)
+    int seglen, h, w, C, nhwc, mode, y1, y2, x1, x2, K;
+    float w_prev, w_cur;       // fl32(1 - lam), fl32(lam)
+    float fill[4];
+};
+
+// The erase box of sample j: on, and whether it is valid (include/dmlb.h: an invalid box makes the sample NaN).
+struct EraseBox {
+    int top, left, bh, bw, on, bad;
+    __device__ __forceinline__ EraseBox(const MixArgs &a, long long j) {
+        top = left = bh = bw = on = bad = 0;
+        if (a.erase) {
+            const int *e = a.erase + 5 * j;
+            top = __ldg(e), left = __ldg(e + 1), bh = __ldg(e + 2), bw = __ldg(e + 3), on = __ldg(e + 4) != 0;
+            bad = on && !(top >= 0 && left >= 0 && bh >= 0 && bw >= 0 && top <= a.h - bh && left <= a.w - bw);
+        }
+    }
+    __device__ __forceinline__ bool covers(int y, int x) const {
+        return on && (unsigned)(y - top) < (unsigned)bh && (unsigned)(x - left) < (unsigned)bw;
+    }
+};
+
+template <int V>
+__device__ __forceinline__ void mix_load(const float *p, float *v) {
+    if constexpr (V == 1) {
+        v[0] = __ldg(p);
+    } else {
+#pragma unroll
+        for (int q = 0; q < V / 4; ++q) {
+            const uint4 u = ld_stream_u4(reinterpret_cast<const uint4 *>(p) + q);
+            v[4 * q] = __uint_as_float(u.x), v[4 * q + 1] = __uint_as_float(u.y);
+            v[4 * q + 2] = __uint_as_float(u.z), v[4 * q + 3] = __uint_as_float(u.w);
+        }
+    }
+}
+
+template <bool kBf16, int V>
+__device__ __forceinline__ void mix_store(void *out, long long e, const float *v) {
+    if constexpr (V == 1) {
+        if (kBf16)
+            reinterpret_cast<uint16_t *>(out)[e] = f32_to_bf16(v[0]);
+        else
+            reinterpret_cast<float *>(out)[e] = v[0];
+    } else if constexpr (kBf16) {
+        static_assert(V == 8, "bf16 stores take 8 values");
+        *reinterpret_cast<uint4 *>(reinterpret_cast<uint16_t *>(out) + e) =
+            make_uint4(pack_bf16x2(v[0], v[1]), pack_bf16x2(v[2], v[3]), pack_bf16x2(v[4], v[5]), pack_bf16x2(v[6], v[7]));
+    } else {
+        static_assert(V == 4, "fp32 stores take 4 values");
+        *reinterpret_cast<float4 *>(reinterpret_cast<float *>(out) + e) = make_float4(v[0], v[1], v[2], v[3]);
+    }
+}
+
+template <bool kBf16, int V>
+__global__ void __launch_bounds__(kMixThreads) image_mix_kernel(const MixArgs a) {
+    const long long pos = (long long)blockIdx.x * kMixThreads + threadIdx.x;
+    const long long B = a.batch;
+    if (pos < a.nvec) {
+        const long long p0 = pos * V;
+        // (y, x) and the fill of each owned element: fixed for the whole walk
+        int ys[V], xs[V];
+        float fv[V];
+        uint32_t cut = 0;  // bit k: element k lies in the CutMix box
+#pragma unroll
+        for (int k = 0; k < V; ++k) {
+            const long long p = p0 + k;
+            int c, pix;
+            if (a.nhwc) {
+                pix = (int)(p / a.C), c = (int)(p - (long long)pix * a.C);
+            } else {
+                const int plane = a.h * a.w;
+                c = (int)(p / plane), pix = (int)(p - (long long)c * plane);
+            }
+            ys[k] = pix / a.w, xs[k] = pix - ys[k] * a.w;
+            fv[k] = a.fill[c];
+            if (ys[k] >= a.y1 && ys[k] < a.y2 && xs[k] >= a.x1 && xs[k] < a.x2) cut |= 1u << k;
+        }
+        // the erased values of sample j, and whether they are NaN (an invalid erase box)
+        auto erased = [&](long long j, float *v) {
+            mix_load<V>(a.src + j * a.S + p0, v);
+            const EraseBox box(a, j);
+#pragma unroll
+            for (int k = 0; k < V; ++k)
+                if (box.covers(ys[k], xs[k])) v[k] = fv[k];
+            return box.bad;
+        };
+        const long long i0 = (long long)blockIdx.y * a.seglen;
+        const long long i1 = min(i0 + (long long)a.seglen, B);
+        float prev[V];
+        int prev_bad = 0;
+        if (a.mode != 0 && i0 < i1) prev_bad = erased(i0 == 0 ? B - 1 : i0 - 1, prev);
+        for (long long i = i0; i < i1; i += kMixUnroll) {
+            float cur[kMixUnroll][V];
+            int bad[kMixUnroll];
+#pragma unroll
+            for (int u = 0; u < kMixUnroll; ++u)
+                if (i + u < i1) bad[u] = erased(i + u, cur[u]);
+#pragma unroll
+            for (int u = 0; u < kMixUnroll; ++u) {
+                if (i + u >= i1) break;
+                float o[V];
+#pragma unroll
+                for (int k = 0; k < V; ++k) {
+                    bool nan = bad[u];
+                    if (a.mode == 1) {
+                        o[k] = __fadd_rn(__fmul_rn(prev[k], a.w_prev), __fmul_rn(cur[u][k], a.w_cur));
+                        nan = nan || prev_bad;
+                    } else if (a.mode == 2 && ((cut >> k) & 1u)) {
+                        o[k] = prev[k];
+                        nan = prev_bad;
+                    } else {
+                        o[k] = cur[u][k];
+                    }
+                    if (nan) o[k] = __uint_as_float(0x7fc00000u);
+                }
+                mix_store<kBf16, V>(a.out, (i + u) * a.S + p0, o);
+#pragma unroll
+                for (int k = 0; k < V; ++k) prev[k] = cur[u][k];
+                prev_bad = bad[u];
+            }
+        }
+    }
+    // the targets: int64 labels (mode 0) or soft targets [B][K]
+    const long long nthreads = (long long)gridDim.x * gridDim.y * kMixThreads;
+    const long long t0 = ((long long)blockIdx.y * gridDim.x + blockIdx.x) * kMixThreads + threadIdx.x;
+    if (a.mode == 0) {
+        for (long long i = t0; i < B; i += nthreads)
+            reinterpret_cast<long long *>(a.targets)[i] = a.labels[a.idx[i]];
+        return;
+    }
+    auto soft = [&](long long e) {
+        const long long i = e / a.K;
+        const long long k = e - i * a.K;
+        const long long cur = a.labels[a.idx[i]], prv = a.labels[a.idx[i == 0 ? B - 1 : i - 1]];
+        if (cur < 0 || cur >= a.K || prv < 0 || prv >= a.K) return __uint_as_float(0x7fc00000u);
+        return __fadd_rn(__fmul_rn(prv == k ? 1.0f : 0.0f, a.w_prev), __fmul_rn(cur == k ? 1.0f : 0.0f, a.w_cur));
+    };
+    float *t = reinterpret_cast<float *>(a.targets);
+    const long long n = B * a.K;
+    const long long head = min(n, (long long)(((16u - ((uint32_t)(uintptr_t)t & 15u)) & 15u) / 4));
+    const long long nv = (n - head) / 4, tail0 = head + 4 * nv;
+    for (long long q = t0; q < nv; q += nthreads) {
+        const long long e = head + 4 * q;
+        *reinterpret_cast<float4 *>(t + e) = make_float4(soft(e), soft(e + 1), soft(e + 2), soft(e + 3));
+    }
+    for (long long q = t0; q < head + (n - tail0); q += nthreads) {
+        const long long e = q < head ? q : tail0 + (q - head);
+        t[e] = soft(e);
+    }
+}
+
+template <bool kBf16, int V>
+static int launch_mix(dim3 grid, cudaStream_t st, const MixArgs &a) {
+    image_mix_kernel<kBf16, V><<<grid, kMixThreads, 0, st>>>(a);
+    return launched();
+}
+
 }  // namespace dmlb
 
 using namespace dmlb;
@@ -642,6 +817,52 @@ int dmlb_image_resample_u8(const uint8_t *images, const int64_t *idx, const int3
                              : launch_resample<true, false>(grid, p.smem, st, a);
     return channels_last ? launch_resample<false, true>(grid, p.smem, st, a)
                          : launch_resample<false, false>(grid, p.smem, st, a);
+}
+
+int dmlb_image_mix(const float *src, const int64_t *idx, const int64_t *labels, const int32_t *erase, const float *fill,
+                   int64_t batch, int32_t C, int32_t h, int32_t w, int mode, double lam, int32_t y1, int32_t y2,
+                   int32_t x1, int32_t x2, int32_t num_classes, void *out, int out_bf16, int channels_last,
+                   void *targets, void *stream) {
+    if (batch < 0 || C < 1 || C > 4 || h < 1 || w < 1 || h > kMixMaxSide || w > kMixMaxSide) return DMLB_EINVAL;
+    if (mode < 0 || mode > 2 || !(lam >= 0.0 && lam <= 1.0)) return DMLB_EINVAL;
+    if (y1 < 0 || y1 > y2 || y2 > h || x1 < 0 || x1 > x2 || x2 > w) return DMLB_EINVAL;
+    if (mode != 0 && num_classes < 1) return DMLB_EINVAL;
+    if (batch > 0 && (!src || !idx || !labels || !out || !targets || (erase && !fill))) return DMLB_EINVAL;
+    const long long S = (long long)C * h * w;
+    if (((uintptr_t)out & (out_bf16 ? 1 : 3)) != 0 || ((uintptr_t)src & 3) != 0 || ((uintptr_t)erase & 3) != 0 ||
+        ((uintptr_t)targets & (mode == 0 ? 7 : 3)) != 0)
+        return DMLB_EALIGN;
+    if (batch == 0) return DMLB_OK;
+
+    MixArgs a;
+    a.src = src;
+    a.idx = (const long long *)idx;
+    a.labels = (const long long *)labels;
+    a.erase = erase;
+    a.out = out;
+    a.targets = targets;
+    a.batch = batch;
+    a.S = S;
+    a.h = h, a.w = w, a.C = C, a.nhwc = channels_last ? 1 : 0, a.mode = mode;
+    a.y1 = mode == 2 ? y1 : 0, a.y2 = mode == 2 ? y2 : 0, a.x1 = mode == 2 ? x1 : 0, a.x2 = mode == 2 ? x2 : 0;
+    a.K = mode == 0 ? 1 : num_classes;
+    a.w_prev = (float)(1.0 - lam);
+    a.w_cur = (float)lam;
+    for (int c = 0; c < 4; ++c) a.fill[c] = erase && c < C ? fill[c] : 0.0f;
+    const int V = out_bf16 ? 8 : 4;
+    const bool vec = S % V == 0 && ((uintptr_t)src & 15) == 0 && ((uintptr_t)out & 15) == 0;
+    a.nvec = vec ? S / V : S;
+    // segments: enough of them to give every SM kMixCtasPerSm CTAs, none shorter than one unrolled group
+    const long long gx = (a.nvec + kMixThreads - 1) / kMixThreads;
+    long long nseg = ((long long)sm_count() * kMixCtasPerSm + gx - 1) / gx;
+    const long long max_seg = (batch + kMixUnroll - 1) / kMixUnroll;
+    nseg = nseg < max_seg ? nseg : max_seg;  // at most sm_count * kMixCtasPerSm, far below the grid's y limit
+    a.seglen = (int)((batch + nseg - 1) / nseg);
+    nseg = (batch + a.seglen - 1) / a.seglen;
+    const dim3 grid((unsigned)gx, (unsigned)nseg);  // gx <= 2^32 / 256 at the largest accepted sample
+    cudaStream_t st = (cudaStream_t)stream;
+    if (out_bf16) return vec ? launch_mix<true, 8>(grid, st, a) : launch_mix<true, 1>(grid, st, a);
+    return vec ? launch_mix<false, 4>(grid, st, a) : launch_mix<false, 1>(grid, st, a);
 }
 
 }  // extern "C"

@@ -16,6 +16,8 @@ gather + normalise kernel (libdmlb dmlb_shard_gather_u8) instead of a host DataL
 per-channel normalisation in one kernel (dmlb_image_batch_u8), and `DeviceResizedImageDataset` does the ImageNet
 recipes (RandomResizedCrop or Resize + CenterCrop, flip, normalise) with one resampling kernel (dmlb_image_resample_u8).
 """
+import ctypes
+import math
 from concurrent.futures import ThreadPoolExecutor
 from typing import Iterable, Sequence
 
@@ -284,11 +286,26 @@ class DeviceImageDataset(DeviceShardedDataset):
     the centre window (validation).  A sample's window and flip depend only on (aug_seed, epoch, its dataset index), so
     they are the same at every rank and world size; set_epoch advances the shard permutation and the augmentation
     together.  Sharding, shuffle, even_shards and drop_last are DeviceShardedDataset's.
+
+    Batch mixing (torchvision v2's classification recipe after Normalize; every argument off by default):
+      random_erase  RandomErasing(p=random_erase, scale=erase_scale, ratio=erase_ratio, value=erase_value) on every
+                    sample; value is a number or one per channel ('random' is refused).  The boxes depend only on
+                    (aug_seed, epoch, dataset index), like the crops (erase_boxes).
+      mixup_alpha, cutmix_alpha   RandomChoice([MixUp(mixup_alpha), CutMix(cutmix_alpha)]) on every batch (only the one
+                    whose alpha is > 0 when the other is 0), with num_classes one-hot targets.  The choice and the draws
+                    depend on (aug_seed, epoch, rank, batch number): batches are rank-local, so unlike the crops these
+                    differ between ranks and world sizes (mix_batch_params).
+    With either alpha > 0 the batches are (x, targets), targets fp32 [B, num_classes] (label smoothing belongs to the
+    loss, as in torchvision); with erasing alone they are (x, int64 y).  Either way each batch is two launches: the image
+    kernel writes an fp32 scratch batch and dmlb_image_mix erases, mixes and writes x and the targets.
+    mix_params() gives the erase table and the per-batch draws of the epoch.
     """
 
     def __init__(self, images, labels, batch_size, mean, std, crop=None, padding=0, random_crop=True, hflip=False,
                  memory_format=torch.contiguous_format, out_dtype=torch.float32, shuffle=True, even_shards=True, seed=0,
-                 aug_seed=None, rank=None, world_size=None, device=None, drop_last=False):
+                 aug_seed=None, rank=None, world_size=None, device=None, drop_last=False, mixup_alpha=0.0,
+                 cutmix_alpha=0.0, num_classes=None, random_erase=0.0, erase_scale=(0.02, 0.33), erase_ratio=(0.3, 3.3),
+                 erase_value=0.0):
         if images.dim() != 4 or not 1 <= images.shape[3] <= 4:
             raise ValueError('images must be uint8 [N, H, W, C] with 1 <= C <= 4')
         if memory_format not in (torch.contiguous_format, torch.channels_last):
@@ -312,6 +329,110 @@ class DeviceImageDataset(DeviceShardedDataset):
         self.memory_format = memory_format
         self.aug_seed = seed if aug_seed is None else aug_seed
         self._norm = self._N.ImageNorm.of(mean, std)
+        self._init_mixing(mixup_alpha, cutmix_alpha, num_classes, random_erase, erase_scale, erase_ratio, erase_value)
+
+    def _init_mixing(self, mixup_alpha, cutmix_alpha, num_classes, random_erase, erase_scale, erase_ratio, erase_value):
+        C = self.item_shape[2]
+        self.mixup_alpha, self.cutmix_alpha = float(mixup_alpha), float(cutmix_alpha)
+        if not (self.mixup_alpha >= 0.0 and self.cutmix_alpha >= 0.0):
+            raise ValueError(f'mixup_alpha and cutmix_alpha must be >= 0, got {mixup_alpha}, {cutmix_alpha}')
+        mixing = self.mixup_alpha > 0.0 or self.cutmix_alpha > 0.0
+        self.num_classes = None if num_classes is None else int(num_classes)
+        if mixing:
+            if self.num_classes is None or self.num_classes < 1:
+                raise ValueError('MixUp and CutMix need num_classes >= 1 for their one-hot targets')
+            if self.labels.numel() and not (int(self.labels.min()) >= 0 and int(self.labels.max()) < self.num_classes):
+                raise ValueError(f'labels must lie in [0, num_classes = {self.num_classes})')
+        self.random_erase = float(random_erase)
+        if not 0.0 <= self.random_erase <= 1.0:
+            raise ValueError(f'random_erase is a probability in [0, 1], got {random_erase}')
+        self.erase_scale, self.erase_ratio = tuple(float(v) for v in erase_scale), tuple(float(v) for v in erase_ratio)
+        if len(self.erase_scale) != 2 or not 0.0 <= self.erase_scale[0] <= self.erase_scale[1] <= 1.0:
+            raise ValueError(f'erase_scale must satisfy 0 <= scale[0] <= scale[1] <= 1, got {erase_scale}')
+        if len(self.erase_ratio) != 2 or not 0.0 < self.erase_ratio[0] <= self.erase_ratio[1] < math.inf:
+            raise ValueError(f'erase_ratio must satisfy 0 < ratio[0] <= ratio[1], got {erase_ratio}')
+        if isinstance(erase_value, str):
+            raise ValueError("erase_value='random' is not supported: its normal draws cannot be reproduced")
+        value = [float(erase_value)] if np.ndim(erase_value) == 0 else [float(v) for v in erase_value]
+        if len(value) not in (1, C):
+            raise ValueError(f'erase_value needs one value or one per channel ({C}), got {len(value)}')
+        self.erase_value = value * C if len(value) == 1 else value
+        self._fill = (ctypes.c_float * 4)(*(self.erase_value + [0.0] * (4 - C)))
+        self._mixing = mixing or self.random_erase > 0.0
+        if self._mixing and max(self.crop) > 32768:
+            raise ValueError(f'crop {self.crop}: dmlb_image_mix takes sides of at most 32768')
+
+    def _shard_rows(self):
+        """This rank's dataset rows for the current epoch in iteration order (numpy)."""
+        return self._epoch_order()[self.rank::self.world_size][:self.shard_len()]
+
+    def epoch_erase_boxes(self):
+        """int32 [shard_len(), 5] numpy {top, left, height, width, erased} of this rank's samples this epoch, in
+        iteration order, in output pixels (erase_boxes; all zero when random_erase is 0)."""
+        rows = self._shard_rows()
+        if self.random_erase <= 0.0:
+            return np.zeros((len(rows), 5), dtype=np.int32)
+        return erase_boxes(rows, self.crop[0], self.crop[1], self.random_erase, self.erase_scale, self.erase_ratio,
+                           self.aug_seed, self.epoch)
+
+    def batch_params(self, batch):
+        """{'mode', 'lam', 'lam_adjusted', 'box'} of this rank's batch number `batch` this epoch (mix_batch_params)."""
+        return mix_batch_params(self.aug_seed, self.epoch, self.rank, batch, self.crop[0], self.crop[1],
+                                self.mixup_alpha, self.cutmix_alpha)
+
+    def mix_params(self):
+        """(indices, erase, batches): this rank's dataset indices for the current epoch in iteration order, the device
+        int32 [count, 5] erase table and the batch_params() of every batch, as the batches of this epoch use them."""
+        return (self.epoch_indices(), torch.from_numpy(self.epoch_erase_boxes()).to(self.device),
+                [self.batch_params(n) for n in range(len(self))])
+
+    def _mixed(self, view, scratch, erase, batch):
+        """Erase, mix and write the batch of the rows `view` from its fp32 `scratch` (one dmlb_image_mix launch)."""
+        N = self._N
+        _, _, C = self.item_shape
+        h, w = self.crop
+        b = view.numel()
+        p = self.batch_params(batch)
+        x = self._empty(b)
+        if p['mode']:
+            y = torch.empty((b, self.num_classes), dtype=torch.float32, device=self.device)
+        else:
+            y = torch.empty(b, dtype=torch.int64, device=self.device)
+        x1, y1, x2, y2 = p['box']
+        N.check(N.cuda_lib(self.device.index).dmlb_image_mix(
+            scratch.data_ptr(), view.data_ptr(), self.labels.data_ptr(), None if erase is None else erase.data_ptr(),
+            self._fill, b, C, h, w, p['mode'], p['lam_adjusted'], y1, y2, x1, x2, self.num_classes or 0, x.data_ptr(),
+            int(self.out_dtype == torch.bfloat16), int(self.memory_format == torch.channels_last), y.data_ptr(),
+            N.stream_ptr()), 'image_mix')
+        return x, y
+
+    def _batches(self, idx, launch):
+        """The epoch's batches of the rows `idx`: launch(start, view, x) writes the images of idx[start:start + len(view)]
+        into x, then the labels are gathered, or (batch mixing) x is an fp32 scratch batch that dmlb_image_mix erases
+        and mixes into the yielded batch together with its targets."""
+        N = self._N
+        lib = N.cuda_lib(self.device.index)
+        count = idx.numel()
+        erase = None
+        if self._mixing and self.random_erase > 0.0:
+            erase = torch.from_numpy(self.epoch_erase_boxes()).to(self.device)
+        for start in range(0, count, self.batch_size):
+            b = min(self.batch_size, count - start)
+            if b < self.batch_size and self.drop_last:
+                return
+            view = idx[start:start + b]
+            if self._mixing:
+                scratch = self._empty(b, torch.float32)
+                launch(start, view, scratch)
+                yield self._mixed(view, scratch, None if erase is None else erase[start:start + b],
+                                  start // self.batch_size)
+                continue
+            x = self._empty(b)
+            y = torch.empty(b, dtype=torch.int64, device=self.device)
+            launch(start, view, x)
+            N.check(lib.dmlb_shard_gather_i64(self.labels.data_ptr(), view.data_ptr(), b, y.data_ptr(), N.stream_ptr()),
+                    'shard_gather_i64')
+            yield x, y
 
     def _launch(self, idx, x, params=None):
         N = self._N
@@ -320,17 +441,18 @@ class DeviceImageDataset(DeviceShardedDataset):
         N.check(lib.dmlb_image_batch_u8(self.images.data_ptr(), idx.data_ptr(), idx.numel(), H, W, C, self.crop[0],
                                         self.crop[1], self.padding, int(self.random_crop), int(self.hflip),
                                         self.aug_seed % (1 << 64), self.epoch, self._norm, x.data_ptr(),
-                                        int(self.out_dtype == torch.bfloat16),
+                                        int(x.dtype == torch.bfloat16),
                                         int(self.memory_format == torch.channels_last),
                                         None if params is None else params.data_ptr(), N.stream_ptr()),
                 'image_batch_u8')
 
-    def _empty(self, b):
+    def _empty(self, b, dtype=None):
         C = self.item_shape[2]
         h, w = self.crop
+        dtype = self.out_dtype if dtype is None else dtype
         if self.memory_format == torch.channels_last:
-            return torch.empty((b, h, w, C), dtype=self.out_dtype, device=self.device).permute(0, 3, 1, 2)
-        return torch.empty((b, C, h, w), dtype=self.out_dtype, device=self.device)
+            return torch.empty((b, h, w, C), dtype=dtype, device=self.device).permute(0, 3, 1, 2)
+        return torch.empty((b, C, h, w), dtype=dtype, device=self.device)
 
     def augment_params(self):
         """(indices, params): this rank's dataset indices for the current epoch in iteration order, and the int32
@@ -343,21 +465,7 @@ class DeviceImageDataset(DeviceShardedDataset):
         return idx, params
 
     def __iter__(self):
-        N = self._N
-        lib = N.cuda_lib(self.device.index)
-        idx = self.epoch_indices()
-        count = idx.numel()
-        for start in range(0, count, self.batch_size):
-            b = min(self.batch_size, count - start)
-            if b < self.batch_size and self.drop_last:
-                return
-            x = self._empty(b)
-            y = torch.empty(b, dtype=torch.int64, device=self.device)
-            view = idx[start:start + b]
-            self._launch(view, x)
-            N.check(lib.dmlb_shard_gather_i64(self.labels.data_ptr(), view.data_ptr(), b, y.data_ptr(), N.stream_ptr()),
-                    'shard_gather_i64')
-            yield x, y
+        yield from self._batches(self.epoch_indices(), lambda start, view, x: self._launch(view, x))
 
 
 _GAMMA = np.uint64(0x9E3779B97F4A7C15)
@@ -371,6 +479,20 @@ def _mix(z):
     return z ^ (z >> np.uint64(31))
 
 
+def _row_hash(rows, seed, epoch):
+    """h = mix(mix(mix(seed + g) ^ (epoch + g)) ^ (row + g)) of every row (uint64 array)."""
+    with np.errstate(over='ignore'):
+        h = _mix(np.uint64(seed % (1 << 64)) + _GAMMA)
+        h = _mix(h ^ (np.uint64(epoch % (1 << 64)) + _GAMMA))
+        return _mix(h ^ (np.asarray(rows, dtype=np.int64).astype(np.uint64) + _GAMMA))
+
+
+def _below(u32, n):
+    """u32 * n >> 32: a uniform 32-bit word mapped onto [0, n)."""
+    with np.errstate(over='ignore'):
+        return ((u32 * np.asarray(n).astype(np.uint64)) >> np.uint64(32)).astype(np.int64)
+
+
 def resized_crop_boxes(rows, H, W, scale, ratio, seed, epoch, hflip):
     """int32 [len(rows), 5] {top, left, height, width, flipped}: torchvision RandomResizedCrop.get_params for every
     row, its uniform draws taken from the counter hash h = mix(mix(mix(seed + g) ^ (epoch + g)) ^ (row + g)), so a box
@@ -380,9 +502,7 @@ def resized_crop_boxes(rows, H, W, scale, ratio, seed, epoch, hflip):
     is torchvision's central fallback.  flipped = mix(h + g) >> 63 when hflip.  fp64 numpy, vectorised over the rows."""
     rows = np.asarray(rows, dtype=np.int64)
     with np.errstate(over='ignore'):
-        h = _mix(np.uint64(seed % (1 << 64)) + _GAMMA)
-        h = _mix(h ^ (np.uint64(epoch % (1 << 64)) + _GAMMA))
-        h = _mix(h ^ (rows.astype(np.uint64) + _GAMMA))
+        h = _row_hash(rows, seed, epoch)
 
         def word(k, sel=slice(None)):
             return _mix(h[sel] + np.uint64(k) * _GAMMA)
@@ -390,8 +510,7 @@ def resized_crop_boxes(rows, H, W, scale, ratio, seed, epoch, hflip):
         def u53(k):
             return (word(k) >> np.uint64(11)).astype(np.float64) * 2.0 ** -53
 
-        def below(u32, n):
-            return ((u32 * n.astype(np.uint64)) >> np.uint64(32)).astype(np.int64)
+        below = _below
 
         in_ratio = W / H
         if in_ratio < min(ratio):
@@ -418,6 +537,136 @@ def resized_crop_boxes(rows, H, W, scale, ratio, seed, epoch, hflip):
     return np.concatenate([box, flip[:, None]], axis=1).astype(np.int32)
 
 
+ERASE_WORD = 32  # the erase words of a row, mix(h + k g) for k in 32..62, follow the crop and flip words (k <= 31)
+
+
+def erase_boxes(rows, h, w, p, scale, ratio, seed, epoch):
+    """int32 [len(rows), 5] {top, left, height, width, erased}: torchvision RandomErasing(p, scale, ratio) on an
+    h x w sample for every row, its uniform draws taken from the row's counter hash h_r of resized_crop_boxes, so a box
+    depends only on (seed, epoch, row).  The row is erased when the 53-bit uniform of mix(h_r + 32 g) is below p; then
+    attempt a (0..9) takes the area fraction from mix(h_r + (33 + 3a) g), the log aspect ratio from mix(h_r + (34 + 3a) g)
+    and the offsets from mix(h_r + (35 + 3a) g) (top from its low, left from its high 32 bits, u32 * n >> 32), with
+    make_params' arithmetic: height = round(sqrt(area * aspect)), width = round(sqrt(area / aspect)), halves to even,
+    accepted when height < h and width < w.  After 10 failed attempts, or when not erased, the row is {0, 0, 0, 0, 0}.
+    fp64 numpy, vectorised over the rows."""
+    rows = np.asarray(rows, dtype=np.int64)
+    box = np.zeros((len(rows), 5), dtype=np.int64)
+    with np.errstate(over='ignore'):
+        hr = _row_hash(rows, seed, epoch)
+
+        def word(k, sel=slice(None)):
+            return _mix(hr[sel] + np.uint64(ERASE_WORD + k) * _GAMMA)
+
+        def u53(k):
+            return (word(k) >> np.uint64(11)).astype(np.float64) * 2.0 ** -53
+
+        todo = u53(0) < p
+        lr0, lr1 = np.log(ratio[0]), np.log(ratio[1])
+        for a in range(10):
+            area = h * w * (scale[0] + (scale[1] - scale[0]) * u53(1 + 3 * a))
+            aspect = np.exp(lr0 + (lr1 - lr0) * u53(2 + 3 * a))
+            eh = np.rint(np.sqrt(area * aspect)).astype(np.int64)
+            ew = np.rint(np.sqrt(area / aspect)).astype(np.int64)
+            ok = todo & (eh < h) & (ew < w)
+            if ok.any():
+                off = word(3 + 3 * a, ok)
+                box[ok] = np.stack([_below(off & np.uint64(0xFFFFFFFF), h - eh[ok] + 1),
+                                    _below(off >> np.uint64(32), w - ew[ok] + 1), eh[ok], ew[ok],
+                                    np.ones(int(ok.sum()), dtype=np.int64)], axis=-1)
+                todo &= ~ok
+    return box.astype(np.int32)
+
+
+_M64 = (1 << 64) - 1
+_G = int(_GAMMA)
+MIXUP, CUTMIX = 1, 2
+
+
+def _mix_int(z):
+    """_mix on one python int."""
+    z &= _M64
+    z = ((z ^ (z >> 30)) * 0xBF58476D1CE4E5B9) & _M64
+    z = ((z ^ (z >> 27)) * 0x94D049BB133111EB) & _M64
+    return z ^ (z >> 31)
+
+
+def batch_hash(seed, epoch, rank, batch):
+    """hb = mix(mix(e ^ (rank + g + 2^63)) ^ (batch + g)), e = mix(mix(seed + g) ^ (epoch + g)).  A row's hash is
+    mix(e ^ (row + g)) with row < 2^63, and mix is a bijection, so no rank's word is ever a row's."""
+    e = _mix_int(_mix_int(seed + _G) ^ ((epoch + _G) & _M64))
+    return _mix_int(_mix_int(e ^ ((rank + _G + (1 << 63)) & _M64)) ^ ((batch + _G) & _M64))
+
+
+def _gamma(alpha, uniform):
+    """Gamma(alpha, 1) by Marsaglia and Tsang (2000), with the u^(1/alpha) boost for alpha < 1; `uniform()` gives the
+    next (0, 1] uniform, normals are Box-Muller (one per two uniforms)."""
+    a = alpha + 1.0 if alpha < 1.0 else alpha
+    d = a - 1.0 / 3.0
+    c = 1.0 / math.sqrt(9.0 * d)
+    while True:
+        x = math.sqrt(-2.0 * math.log(uniform())) * math.cos(2.0 * math.pi * uniform())
+        v = 1.0 + c * x
+        if v <= 0.0:
+            continue
+        v = v * v * v
+        if math.log(uniform()) < 0.5 * x * x + d - d * v + d * math.log(v):
+            g = d * v
+            break
+    return g * uniform() ** (1.0 / alpha) if alpha < 1.0 else g
+
+
+def beta_sample(alpha, uniform):
+    """lambda ~ Beta(alpha, alpha) = X / (X + Y), X and Y Gamma(alpha) drawn in that order."""
+    x = _gamma(alpha, uniform)
+    y = _gamma(alpha, uniform)
+    return x / (x + y)
+
+
+def cutmix_box(lam, r_x, r_y, h, w):
+    """((x1, y1, x2, y2), lam_adjusted) of torchvision CutMix.make_params for the draws (lam, r_x, r_y)."""
+    r = 0.5 * math.sqrt(1.0 - lam)
+    r_w_half, r_h_half = int(r * w), int(r * h)
+    x1, y1 = max(r_x - r_w_half, 0), max(r_y - r_h_half, 0)
+    x2, y2 = min(r_x + r_w_half, w), min(r_y + r_h_half, h)
+    return (x1, y1, x2, y2), float(1.0 - (x2 - x1) * (y2 - y1) / (w * h))
+
+
+def mix_batch_params(seed, epoch, rank, batch, h, w, mixup_alpha, cutmix_alpha):
+    """{'mode', 'lam', 'lam_adjusted', 'box'} of batch number `batch` of `rank` in `epoch`: torchvision
+    RandomChoice([MixUp(mixup_alpha), CutMix(cutmix_alpha)]) on an h x w batch, its draws taken from the words
+    mix(hb + k g) of batch_hash (the batches are rank-local, so these draws depend on the rank).
+      mode   MIXUP or CUTMIX when only that alpha is > 0; with both, MIXUP + (mix(hb + g) >> 63); 0 when neither is
+      lam    Beta(alpha, alpha) of the chosen mode (beta_sample), its (0, 1] uniforms ((mix(hb + k g) >> 11) + 1) 2^-53
+             for k = 3, 4, ...
+      box    CutMix's (x1, y1, x2, y2) (cutmix_box) for r_x = lo32(w2) * w >> 32, r_y = hi32(w2) * h >> 32,
+             w2 = mix(hb + 2 g); (0, 0, 0, 0) for MixUp
+      lam_adjusted   the weight of the targets: CutMix's lam_adjusted, MixUp's lam."""
+    if mixup_alpha <= 0.0 and cutmix_alpha <= 0.0:
+        return {'mode': 0, 'lam': 1.0, 'lam_adjusted': 1.0, 'box': (0, 0, 0, 0)}
+    hb = batch_hash(seed, epoch, rank, batch)
+
+    def word(k):
+        return _mix_int((hb + k * _G) & _M64)
+
+    if mixup_alpha > 0.0 and cutmix_alpha > 0.0:
+        mode = MIXUP + (word(1) >> 63)
+    else:
+        mode = MIXUP if mixup_alpha > 0.0 else CUTMIX
+    k = [3]
+
+    def uniform():
+        u = ((word(k[0]) >> 11) + 1) * 2.0 ** -53
+        k[0] += 1
+        return u
+
+    lam = beta_sample(mixup_alpha if mode == MIXUP else cutmix_alpha, uniform)
+    if mode == MIXUP:
+        return {'mode': mode, 'lam': lam, 'lam_adjusted': lam, 'box': (0, 0, 0, 0)}
+    w2 = word(2)
+    box, lam_adjusted = cutmix_box(lam, ((w2 & 0xFFFFFFFF) * w) >> 32, ((w2 >> 32) * h) >> 32, h, w)
+    return {'mode': mode, 'lam': lam, 'lam_adjusted': lam_adjusted, 'box': box}
+
+
 class DeviceResizedImageDataset(DeviceImageDataset):
     """Device-resident colour-image dataset with the ImageNet recipes (SURVEY §8f-1), one resampling launch per batch
     (dmlb_image_resample_u8) plus the label gather.
@@ -431,16 +680,20 @@ class DeviceResizedImageDataset(DeviceImageDataset):
     they are the same at every rank and world size.  Sharding, shuffle, even_shards and drop_last are
     DeviceShardedDataset's.  The kernel takes image and resized sides of at most 32768, resizes at
     most 8x down on each axis and writes rows of at most 1024 values; the constructor refuses anything else.
+    Batch mixing (random_erase, mixup_alpha, cutmix_alpha, ...) is DeviceImageDataset's, on the size[0] x size[1] output.
     """
 
     def __init__(self, images, labels, batch_size, mean, std, size, scale=(0.08, 1.0), ratio=(3 / 4, 4 / 3),
                  random=True, resize=None, hflip=False, memory_format=torch.contiguous_format,
                  out_dtype=torch.float32, shuffle=True, even_shards=True, seed=0, aug_seed=None, rank=None,
-                 world_size=None, device=None, drop_last=False):
+                 world_size=None, device=None, drop_last=False, mixup_alpha=0.0, cutmix_alpha=0.0, num_classes=None,
+                 random_erase=0.0, erase_scale=(0.02, 0.33), erase_ratio=(0.3, 3.3), erase_value=0.0):
         super().__init__(images, labels, batch_size, mean, std, crop=None, padding=0, random_crop=random, hflip=hflip,
                          memory_format=memory_format, out_dtype=out_dtype, shuffle=shuffle, even_shards=even_shards,
                          seed=seed, aug_seed=aug_seed, rank=rank, world_size=world_size, device=device,
-                         drop_last=drop_last)
+                         drop_last=drop_last, mixup_alpha=mixup_alpha, cutmix_alpha=cutmix_alpha,
+                         num_classes=num_classes, random_erase=random_erase, erase_scale=erase_scale,
+                         erase_ratio=erase_ratio, erase_value=erase_value)
         H, W, C = self.item_shape
         size = (int(size), int(size)) if isinstance(size, (int, np.integer)) else tuple(int(v) for v in size)
         if len(size) != 2 or min(size) < 1:
@@ -475,7 +728,7 @@ class DeviceResizedImageDataset(DeviceImageDataset):
         """int32 [shard_len(), 5] numpy {top, left, height, width, flipped} of this rank's samples this epoch, in
         iteration order."""
         H, W, _ = self.item_shape
-        rows = self._epoch_order()[self.rank::self.world_size][:self.shard_len()]
+        rows = self._shard_rows()
         if self.random_crop:
             return resized_crop_boxes(rows, H, W, self.scale, self.ratio, self.aug_seed, self.epoch, self.hflip)
         boxes = np.tile(np.asarray([0, 0, H, W, 0], dtype=np.int32), (len(rows), 1))
@@ -490,7 +743,7 @@ class DeviceResizedImageDataset(DeviceImageDataset):
         N.check(lib.dmlb_image_resample_u8(self.images.data_ptr(), idx.data_ptr(), boxes.data_ptr(), idx.numel(), H, W,
                                            C, self.resized[0], self.resized[1], self.window[0], self.window[1],
                                            self.crop[0], self.crop[1], self._norm, x.data_ptr(),
-                                           int(self.out_dtype == torch.bfloat16),
+                                           int(x.dtype == torch.bfloat16),
                                            int(self.memory_format == torch.channels_last), N.stream_ptr()),
                 'image_resample_u8')
 
@@ -500,18 +753,5 @@ class DeviceResizedImageDataset(DeviceImageDataset):
         return self.epoch_indices(), torch.from_numpy(self.epoch_boxes()).to(self.device)
 
     def __iter__(self):
-        N = self._N
-        lib = N.cuda_lib(self.device.index)
         idx, boxes = self.augment_params()
-        count = idx.numel()
-        for start in range(0, count, self.batch_size):
-            b = min(self.batch_size, count - start)
-            if b < self.batch_size and self.drop_last:
-                return
-            x = self._empty(b)
-            y = torch.empty(b, dtype=torch.int64, device=self.device)
-            view = idx[start:start + b]
-            self._launch(view, x, boxes[start:start + b])
-            N.check(lib.dmlb_shard_gather_i64(self.labels.data_ptr(), view.data_ptr(), b, y.data_ptr(), N.stream_ptr()),
-                    'shard_gather_i64')
-            yield x, y
+        yield from self._batches(idx, lambda start, view, x: self._launch(view, x, boxes[start:start + view.numel()]))

@@ -424,6 +424,50 @@ int dmlb_image_resample_u8(const uint8_t *images, const int64_t *idx, const int3
                            int32_t out_h, int32_t out_w, const dmlb_image_norm *norm, void *out, int out_bf16,
                            int channels_last, void *stream);
 
+/* Batch mixing: random erasing per sample, then MixUp or CutMix over the batch, then the targets, one launch.
+ * torchvision v2's RandomErasing(value=fill) on every sample, then MixUp or CutMix (pairing sample i with i - 1 mod
+ * batch, torchvision's roll(1, 0)), and their one_hot targets mixed by _BaseMixUpCutMix._mixup_label.
+ *   src     : DEVICE fp32 logical [batch, C, h, w] (a batch of dmlb_image_batch_u8 or dmlb_image_resample_u8 written in
+ *             fp32), NCHW (channels_last == 0) or NHWC in memory; out has the same layout, fp32 or bf16 (RNE)
+ *   idx     : DEVICE int64 [batch], the dataset rows of the batch; labels: DEVICE int64 [n], the dataset's labels
+ *   erase   : DEVICE int32 [batch][5] {top, left, height, width, erased} in output pixels, or NULL (nothing erased);
+ *             fill : HOST float [C], the erasing value of each channel (needed when erase is not NULL)
+ * e_i[c, y, x] = fill[c] when erased_i != 0 and top_i <= y < top_i + height_i and left_i <= x < left_i + width_i,
+ *             src[i, c, y, x] otherwise; p = i - 1 (batch - 1 for i = 0; a batch of one pairs a sample with itself)
+ *   mode 0 (none)   : out_i = e_i;                         targets = int64 [batch], targets[i] = labels[idx[i]]
+ *   mode 1 (MixUp)  : out_i = fl32(fl32(e_p * fl32(1 - lam)) + fl32(e_i * fl32(lam)))
+ *   mode 2 (CutMix) : out_i[c, y, x] = e_p[c, y, x] when y1 <= y < y2 and x1 <= x < x2, e_i[c, y, x] otherwise
+ *   modes 1 and 2   : targets = fp32 [batch][num_classes], t_i = one_hot(labels[idx[i]]),
+ *                     targets[i] = fl32(fl32(t_p * fl32(1 - lam)) + fl32(t_i * fl32(lam)))
+ *   lam is MixUp's lambda, and CutMix's lam_adjusted = 1 - (x2 - x1)(y2 - y1) / (h w) (both fp64, as python floats);
+ *   every multiply and add is rounded once (no FMA), fl32(1 - lam) and fl32(lam) are rounded from fp64 once: torch's
+ *   fp32 tensor-by-python-scalar arithmetic, bit for bit.  Label smoothing is left to the loss, as in torchvision.
+ * The datasets (util/data.py) sample the arguments on the host from the hash of dmlb_image_batch_u8:
+ *   erase rows  per dataset row, h = the row's hash: erased when u53(mix(h + 32 g)) < p; attempt a (0..9) takes the
+ *               area fraction from mix(h + (33 + 3a) g), the log aspect from mix(h + (34 + 3a) g), the offsets from
+ *               mix(h + (35 + 3a) g) (top low, left high 32 bits) -- words the crop and flip (k <= 31) never use
+ *   per batch   hb = mix(mix(e ^ (rank + g + 2^63)) ^ (batch + g)), e = mix(mix(seed + g) ^ (epoch + g)), never a
+ *               row's hash; the MixUp / CutMix choice from mix(hb + g) >> 63, CutMix's (r_x, r_y) from mix(hb + 2 g),
+ *               lam ~ Beta(alpha, alpha) from Marsaglia-Tsang Gamma draws on the uniforms of mix(hb + k g), k >= 3.
+ * Accepted range (anything else: DMLB_EINVAL, nothing launched): C in 1..4; h, w in 1..32768; mode in 0..2;
+ * 0 <= lam <= 1; 0 <= y1 <= y2 <= h and 0 <= x1 <= x2 <= w (the box is ignored unless mode == 2); num_classes >= 1
+ * when mode != 0; non-NULL src, idx, labels, out and targets when batch > 0, and fill when erase is not NULL.
+ * DMLB_EALIGN: src or erase not aligned to 4 bytes, out not to its element, targets not to its element (8 bytes in
+ * mode 0, 4 otherwise).  Device data is not checked by the host; the kernel defines what it does with it:
+ *   an erase row with erased != 0 whose box is not inside the sample (top, left, height, width >= 0, top + height <= h,
+ *   left + width <= w) makes e_i quiet NaN: every output value that reads e_i (out_i, and out_{i+1}'s partner values
+ *   when mixing) is written as quiet NaN; rows with erased == 0 are ignored;
+ *   a label outside [0, num_classes) when mixing makes t_i quiet NaN: target rows i and i + 1 are quiet NaN.
+ * Traffic: a thread owns 16 bytes of output at one position of a sample and walks a segment of the batch keeping the
+ * previous sample in registers, so src is read once (plus one partner sample per segment) and out written once with
+ * 16-byte stores (scalar stores when C h w is not a multiple of 16 bytes of output, or src / out are not 16-byte
+ * aligned).  Algorithmic bytes/sample: C h w * 4 read + C h w * (4 | 2) written + 20 B of erase row
+ * + num_classes * 4 (or 8) B of targets. */
+int dmlb_image_mix(const float *src, const int64_t *idx, const int64_t *labels, const int32_t *erase, const float *fill,
+                   int64_t batch, int32_t C, int32_t h, int32_t w, int mode, double lam, int32_t y1, int32_t y2,
+                   int32_t x1, int32_t x2, int32_t num_classes, void *out, int out_bf16, int channels_last,
+                   void *targets, void *stream);
+
 #ifdef __cplusplus
 }
 #endif
