@@ -20,7 +20,7 @@ METRIC_OK, METRIC_SPLIT_VOTE, METRIC_LAYOUT, METRIC_TIMEOUT = 0, 1, 2, 3
 SRC_FEED = 7
 FEED_WIDTH = 16
 STEP_METRIC_MAX_CELLS = 1023
-ABI_VERSION = 2
+ABI_VERSION = 3
 IPC_HANDLE_BYTES = 64
 MAX_WORLD = 8
 MAX_FOLD_ENTRIES = 32
@@ -127,9 +127,8 @@ SIGNATURES = {
     'dmlb_shard_gather_u8': (c_int, [c_void_p, c_void_p, c_int64, c_int64, c_float, c_float, c_void_p, c_int, c_void_p]),
     'dmlb_shard_gather_i64': (c_int, [c_void_p, c_void_p, c_int64, c_void_p, c_void_p]),
     'dmlb_shard_slice': (c_int, [c_void_p, c_int64, c_int64, c_int64, c_int64, c_void_p, c_void_p]),
-    'dmlb_image_batch_u8': (c_int, [c_void_p, c_void_p, c_int64, c_int32, c_int32, c_int32, c_int32, c_int32, c_int32,
-                                    c_int, c_int, c_uint64, c_int64, POINTER(ImageNorm), c_void_p, c_int, c_int,
-                                    c_void_p, c_void_p]),
+    'dmlb_image_batch_u8': (c_int, [c_void_p, c_void_p, c_void_p, c_int64, c_int32, c_int32, c_int32, c_int32, c_int32,
+                                    c_int32, POINTER(ImageNorm), c_void_p, c_int, c_int, c_void_p]),
     'dmlb_image_resample_u8': (c_int, [c_void_p, c_void_p, c_void_p, c_int64, c_int32, c_int32, c_int32, c_int32, c_int32,
                                        c_int32, c_int32, c_int32, c_int32, POINTER(ImageNorm), c_void_p, c_int, c_int,
                                        c_void_p]),

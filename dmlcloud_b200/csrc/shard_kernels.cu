@@ -7,6 +7,7 @@
 //   out[i, :] = (float(images[idx[i], :]) / 255 - mean) / std                      784 B read, 3136 (fp32) B written / sample
 // HBM-bound byte work: 16 pixels (one 128-bit load) per thread, 4x 128-bit stores, rows found through idx[] (L2-resident).
 #include <cmath>
+#include <type_traits>
 
 #include "dmlb_common.cuh"
 
@@ -83,52 +84,29 @@ static inline int grid_for(long long work, int threads) {
 }
 
 // ---- colour images: gather + pad + crop + flip + per-channel normalise (dmlb_image_batch_u8) ------------------------
-// One CTA job = one band of up to `rows` output rows of one sample.  The band's window rows are staged into shared memory
+// (include/dmlb.h states the rule.)  One CTA job = one band of up to `rows` output rows of one sample, at the window
+// {top, left, flipped} the host gave it in `windows`.  The band's window rows are staged into shared memory
 // as the 16-byte aligned chunks of the source rows that cover them (so the loads are 128-bit whatever the crop offset),
 // then written out in the output's contiguous order, 16-byte stores for the body of every contiguous run.  Normalised
 // values come from a per-launch [C][256] table in shared memory built with norm_px, so every element is two shared
 // loads and no division.  HBM traffic is the window bytes (plus < 32 B of chunk rounding per row) and the output.
 
-constexpr uint64_t kImageGamma = 0x9e3779b97f4a7c15ull;
 constexpr int kImageThreads = 256;
 constexpr int kImageBandBytes = 24576;  // staged window bytes per CTA (+ the 4 KB table)
-constexpr int kImageCtasPerSm = 6;      // grid cap: what fits one SM at <= 40 registers per thread (ptxas -v)
+constexpr int kImageCtasPerSm = 6;      // grid cap: what fits one SM at <= 40 registers (__launch_bounds__ holds it)
 constexpr int kImageMaxRowBytes = 49152;
-
-__host__ __device__ __forceinline__ uint64_t splitmix64_mix(uint64_t z) {
-    z = (z ^ (z >> 30)) * 0xbf58476d1ce4e5b9ull;
-    z = (z ^ (z >> 27)) * 0x94d049bb133111ebull;
-    return z ^ (z >> 31);
-}
 
 struct ImageArgs {
     const uint8_t *images;
     const long long *idx;
+    const int *windows;
     void *out;
-    int *params;
     long long batch, sample_bytes;
-    unsigned long long seed;
-    long long epoch;
-    int H, W, C, oh, ow, pad, random_crop, hflip;
+    int H, W, C, oh, ow, pad;
+    long long dy, dx;         // a window's top lies in [0, dy], its left in [0, dx] (H + 2 pad may pass INT_MAX)
     int rows, bands, rowcap;  // band height, bands per sample, staged bytes per window row
     float mean[4], std[4];
 };
-
-// The window of one sample, in padded coordinates (include/dmlb.h states the rule).
-__device__ __forceinline__ void image_window(const ImageArgs &a, long long row, int &top, int &left, int &flip) {
-    const int dy = a.H + 2 * a.pad - a.oh, dx = a.W + 2 * a.pad - a.ow;
-    uint64_t h = splitmix64_mix(a.seed + kImageGamma);
-    h = splitmix64_mix(h ^ ((uint64_t)a.epoch + kImageGamma));
-    h = splitmix64_mix(h ^ ((uint64_t)row + kImageGamma));
-    if (a.random_crop) {
-        top = (int)(((uint64_t)(uint32_t)h * (uint64_t)(dy + 1)) >> 32);
-        left = (int)(((uint64_t)(uint32_t)(h >> 32) * (uint64_t)(dx + 1)) >> 32);
-    } else {  // Python round(d / 2): halves go to the even neighbour
-        top = (dy >> 1) + ((dy & 1) & ((dy >> 1) & 1));
-        left = (dx >> 1) + ((dx & 1) & ((dx >> 1) & 1));
-    }
-    flip = a.hflip ? (int)(splitmix64_mix(h + kImageGamma) >> 63) : 0;
-}
 
 // One band of one sample, staged in shared memory: window row r holds source bytes from an address whose low 4 bits are
 // `head(r)` (0 on the byte-load path), columns [u_lo, u_hi) of the window are inside the image, the rest is padding.
@@ -152,7 +130,7 @@ struct ImageBand {
 };
 
 // Walks a contiguous run of output elements in memory order: NCHW runs stay in one channel plane, NHWC runs step c fastest.
-// Band: any band type with members C, ow and value(r, x, c) (ImageBand, ResampleBand).
+// Band: any band type with members C, ow and value(r, x, c) (ImageBand, NanBand, ResampleBand).
 template <class Band, bool kNHWC>
 struct ImageCursor {
     const Band &b;
@@ -199,8 +177,35 @@ __device__ __forceinline__ void image_store_run(void *out, long long first, int 
     }
 }
 
+// Rows [y0, y0 + nr) of sample i of the logical [batch, C, oh, ow] output a.out (plane = oh * ow), written in its
+// memory order (NCHW: one run per channel plane, NHWC: one run) from band.value.  Args: ImageArgs or ResampleArgs.
+template <bool kBf16, bool kNHWC, class Args, class Band>
+__device__ __forceinline__ void store_band(const Args &a, long long i, int y0, int nr, int plane, const Band &band) {
+    if (kNHWC) {
+        const int C = a.C, ow = a.ow;
+        image_store_run<kBf16>(a.out, i * plane * C + (long long)y0 * ow * C, nr * ow * C, [&](int k) {
+            const int p = k / C;
+            return ImageCursor<Band, true>{band, p / ow, p - (p / ow) * ow, k - p * C};
+        });
+    } else {
+        for (int c = 0; c < a.C; ++c) {
+            const int ow = a.ow;
+            image_store_run<kBf16>(a.out, (i * a.C + c) * plane + (long long)y0 * ow, nr * ow, [&](int k) {
+                return ImageCursor<Band, false>{band, k / ow, k - (k / ow) * ow, c};
+            });
+        }
+    }
+}
+
+// The band of a sample whose window lies outside the padded image: quiet NaN, nothing read.
+template <bool kBf16>
+struct NanBand {
+    int C, ow;
+    __device__ __forceinline__ uint32_t value(int, int, int) const { return kBf16 ? 0x7fc0u : 0x7fc00000u; }
+};
+
 template <bool kBf16, bool kNHWC, bool kVecLoad>
-__global__ void __launch_bounds__(kImageThreads) image_batch_u8_kernel(const ImageArgs a) {
+__global__ void __launch_bounds__(kImageThreads, kImageCtasPerSm) image_batch_u8_kernel(const ImageArgs a) {
     extern __shared__ uint4 s_band[];
     __shared__ uint32_t s_lut[4 * 256];
     uint8_t *sm = reinterpret_cast<uint8_t *>(s_band);
@@ -214,14 +219,12 @@ __global__ void __launch_bounds__(kImageThreads) image_batch_u8_kernel(const Ima
         const long long i = job / a.bands;
         const int y0 = (int)(job - i * a.bands) * a.rows;
         const int nr = min(a.rows, a.oh - y0);
-        const long long row = a.idx[i];
-        int top, left, flip;
-        image_window(a, row, top, left, flip);
-        if (a.params && y0 == 0 && threadIdx.x == 0) {
-            a.params[3 * i] = top;
-            a.params[3 * i + 1] = left;
-            a.params[3 * i + 2] = flip;
+        const int top = a.windows[3 * i], left = a.windows[3 * i + 1], flip = a.windows[3 * i + 2] != 0;
+        if (top < 0 || top > a.dy || left < 0 || left > a.dx) {
+            store_band<kBf16, kNHWC>(a, i, y0, nr, plane, NanBand<kBf16>{a.C, a.ow});
+            continue;
         }
+        const long long row = a.idx[i];
         const uint8_t *img = a.images + row * a.sample_bytes;
         const int sx0 = left - a.pad, sy0 = top - a.pad + y0;
         const int u_lo = max(0, -sx0), u_hi = min(a.ow, a.W - sx0);
@@ -256,31 +259,47 @@ __global__ void __launch_bounds__(kImageThreads) image_batch_u8_kernel(const Ima
             }
         }
         __syncthreads();
-        const ImageBand<kVecLoad> band{sm, s_lut, (uint32_t)(uintptr_t)col0, sy0, a.H, WC, a.C, a.ow, u_lo, u_hi,
-                                       a.rowcap, flip};
-        if (kNHWC) {
-            const int C = a.C, ow = a.ow;
-            image_store_run<kBf16>(a.out, i * plane * C + (long long)y0 * ow * C, nr * ow * C, [&](int k) {
-                const int p = k / C;
-                return ImageCursor<ImageBand<kVecLoad>, true>{band, p / ow, p - (p / ow) * ow, k - p * C};
-            });
-        } else {
-            for (int c = 0; c < a.C; ++c) {
-                const int ow = a.ow;
-                image_store_run<kBf16>(a.out, (i * a.C + c) * plane + (long long)y0 * ow, nr * ow, [&](int k) {
-                    return ImageCursor<ImageBand<kVecLoad>, false>{band, k / ow, k - (k / ow) * ow, c};
-                });
-            }
-        }
+        store_band<kBf16, kNHWC>(a, i, y0, nr, plane,
+                                 ImageBand<kVecLoad>{sm, s_lut, (uint32_t)(uintptr_t)col0, sy0, a.H, WC, a.C, a.ow,
+                                                     u_lo, u_hi, a.rowcap, flip});
     }
 }
 
 template <bool kBf16, bool kNHWC>
-static void launch_image(bool vec_load, int grid, size_t smem, cudaStream_t st, const ImageArgs &a) {
+static int launch_image(bool vec_load, int grid, size_t smem, cudaStream_t st, const ImageArgs &a) {
     if (vec_load)
         image_batch_u8_kernel<kBf16, kNHWC, true><<<grid, kImageThreads, smem, st>>>(a);
     else
         image_batch_u8_kernel<kBf16, kNHWC, false><<<grid, kImageThreads, smem, st>>>(a);
+    return launched();
+}
+
+// ---- host scaffolding of the two band kernels -----------------------------------------------------------------------
+
+// Refuses std[c] == 0 for c < C; otherwise fills the kernel's 4-channel mean and std (channels past C: 0 and 1).
+static bool pack_norm(const dmlb_image_norm *norm, int C, float *mean, float *std) {
+    for (int c = 0; c < C; ++c)
+        if (norm->std[c] == 0.0f) return false;
+    for (int c = 0; c < 4; ++c) {
+        mean[c] = c < C ? norm->mean[c] : 0.0f;
+        std[c] = c < C ? norm->std[c] : 1.0f;
+    }
+    return true;
+}
+
+// One CTA per band job, at most ctas_per_sm CTAs per SM (each CTA then walks several jobs).
+static int band_grid(long long jobs, int ctas_per_sm) {
+    const long long cap = (long long)sm_count() * ctas_per_sm;
+    return (int)(jobs < cap ? jobs : cap);
+}
+
+// Returns launch(bf16, nhwc), the two passed as std::bool_constant so that launch can name a kernel instance.
+template <class Launch>
+static int dispatch_layout(int out_bf16, int channels_last, const Launch &launch) {
+    using T = std::true_type;
+    using F = std::false_type;
+    if (out_bf16) return channels_last ? launch(T{}, T{}) : launch(T{}, F{});
+    return channels_last ? launch(F{}, T{}) : launch(F{}, F{});
 }
 
 
@@ -288,7 +307,7 @@ static void launch_image(bool vec_load, int grid, size_t smem, cudaStream_t st, 
 // (dmlb_image_resample_u8; include/dmlb.h states the rule.)  One CTA job = one band of up to `rows` output rows of one
 // sample.  The CTA builds the sample's column taps (xmin, xsize, weights) for the window's columns and the row taps of
 // the band, runs the horizontal pass over the band's source rows into an fp32 [srows][out_w * C] tile in shared memory,
-// then the vertical pass, written in the output's contiguous order by image_store_run.  Source bytes are read through
+// then the vertical pass, written in the output's contiguous order by store_band.  Source bytes are read through
 // L1 (a box row's bytes are read by neighbouring columns' taps) and mapped through a 256-entry fl32(byte) / 255 table.
 // Every operation of the tap and pixel arithmetic is rounded once, as written (no FMA contraction).
 
@@ -429,22 +448,9 @@ __global__ void __launch_bounds__(kResampleThreads) image_resample_u8_kernel(con
             sm.tile[t] = acc;
         }
         __syncthreads();
-        const ResampleBand<kBf16> band{sm.tile, sm.wy, s_norm, s_norm + 4, sm.ymin, sm.ysize, ylo, rowf, a.ky, a.C,
-                                       a.ow, flip, ok};
-        if (kNHWC) {
-            const int C = a.C, ow = a.ow;
-            image_store_run<kBf16>(a.out, i * plane * C + (long long)y0 * ow * C, nr * ow * C, [&](int k) {
-                const int p = k / C;
-                return ImageCursor<ResampleBand<kBf16>, true>{band, p / ow, p - (p / ow) * ow, k - p * C};
-            });
-        } else {
-            for (int c = 0; c < a.C; ++c) {
-                const int ow = a.ow;
-                image_store_run<kBf16>(a.out, (i * a.C + c) * plane + (long long)y0 * ow, nr * ow, [&](int k) {
-                    return ImageCursor<ResampleBand<kBf16>, false>{band, k / ow, k - (k / ow) * ow, c};
-                });
-            }
-        }
+        store_band<kBf16, kNHWC>(a, i, y0, nr, plane,
+                                 ResampleBand<kBf16>{sm.tile, sm.wy, s_norm, s_norm + 4, sm.ymin, sm.ysize, ylo, rowf,
+                                                     a.ky, a.C, a.ow, flip, ok});
     }
 }
 
@@ -720,61 +726,40 @@ int dmlb_shard_slice(const int64_t *perm, int64_t first, int64_t count, int64_t 
     return launched();
 }
 
-int dmlb_image_batch_u8(const uint8_t *images, const int64_t *idx, int64_t batch, int32_t H, int32_t W, int32_t C,
-                        int32_t out_h, int32_t out_w, int32_t pad, int crop_mode, int hflip, uint64_t seed, int64_t epoch,
-                        const dmlb_image_norm *norm, void *out, int out_bf16, int channels_last, int32_t *params_out,
-                        void *stream) {
+int dmlb_image_batch_u8(const uint8_t *images, const int64_t *idx, const int32_t *windows, int64_t batch, int32_t H,
+                        int32_t W, int32_t C, int32_t out_h, int32_t out_w, int32_t pad, const dmlb_image_norm *norm,
+                        void *out, int out_bf16, int channels_last, void *stream) {
     if (batch < 0 || !norm || C < 1 || C > 4 || H < 1 || W < 1 || out_h < 1 || out_w < 1 || pad < 0) return DMLB_EINVAL;
-    if ((crop_mode != 0 && crop_mode != 1) || (long long)out_h > (long long)H + 2LL * pad ||
-        (long long)out_w > (long long)W + 2LL * pad)
-        return DMLB_EINVAL;
-    for (int c = 0; c < C; ++c)
-        if (norm->std[c] == 0.0f) return DMLB_EINVAL;
-    if (batch > 0 && (!images || !idx || !out)) return DMLB_EINVAL;
+    const long long dy = (long long)H + 2LL * pad - out_h, dx = (long long)W + 2LL * pad - out_w;
+    if (dy < 0 || dx < 0) return DMLB_EINVAL;
+    ImageArgs a;
+    if (!pack_norm(norm, C, a.mean, a.std)) return DMLB_EINVAL;
+    if (batch > 0 && (!images || !idx || !windows || !out)) return DMLB_EINVAL;
     const long long rowcap = ((long long)out_w * C + 15) / 16 * 16 + 16;
     if (rowcap > kImageMaxRowBytes) return DMLB_EINVAL;
-    if (((uintptr_t)out & (out_bf16 ? 1 : 3)) != 0) return DMLB_EALIGN;
+    if (((uintptr_t)out & (out_bf16 ? 1 : 3)) != 0 || ((uintptr_t)windows & 3) != 0) return DMLB_EALIGN;
     if (batch == 0) return DMLB_OK;
 
-    ImageArgs a;
     a.images = images;
     a.idx = (const long long *)idx;
+    a.windows = windows;
     a.out = out;
-    a.params = params_out;
     a.batch = batch;
     a.sample_bytes = (long long)H * W * C;
-    a.seed = seed;
-    a.epoch = epoch;
     a.H = H, a.W = W, a.C = C, a.oh = out_h, a.ow = out_w, a.pad = pad;
-    a.random_crop = crop_mode, a.hflip = hflip ? 1 : 0;
+    a.dy = dy, a.dx = dx;
     const int max_rows = (int)(kImageBandBytes / rowcap) > 0 ? (int)(kImageBandBytes / rowcap) : 1;
     a.bands = (out_h + max_rows - 1) / max_rows;
     a.rows = (out_h + a.bands - 1) / a.bands;
     a.rowcap = (int)rowcap;
-    for (int c = 0; c < 4; ++c) {
-        a.mean[c] = c < C ? norm->mean[c] : 0.0f;
-        a.std[c] = c < C ? norm->std[c] : 1.0f;
-    }
-    const long long jobs = batch * a.bands;
-    const long long cap = (long long)sm_count() * kImageCtasPerSm;
-    const int grid = (int)(jobs < cap ? jobs : cap);
+    const int grid = band_grid(batch * a.bands, kImageCtasPerSm);
     const size_t smem = (size_t)a.rows * a.rowcap;
     const bool vec_load = ((uintptr_t)images & 15) == 0;
     cudaStream_t st = (cudaStream_t)stream;
-    if (out_bf16) {
-        if (channels_last)
-            launch_image<true, true>(vec_load, grid, smem, st, a);
-        else
-            launch_image<true, false>(vec_load, grid, smem, st, a);
-    } else {
-        if (channels_last)
-            launch_image<false, true>(vec_load, grid, smem, st, a);
-        else
-            launch_image<false, false>(vec_load, grid, smem, st, a);
-    }
-    return launched();
+    return dispatch_layout(out_bf16, channels_last, [&](auto bf16, auto nhwc) {
+        return launch_image<decltype(bf16)::value, decltype(nhwc)::value>(vec_load, grid, smem, st, a);
+    });
 }
-
 
 int dmlb_image_resample_u8(const uint8_t *images, const int64_t *idx, const int32_t *boxes, int64_t batch, int32_t H,
                            int32_t W, int32_t C, int32_t resize_h, int32_t resize_w, int32_t win_top, int32_t win_left,
@@ -787,14 +772,13 @@ int dmlb_image_resample_u8(const uint8_t *images, const int64_t *idx, const int3
         return DMLB_EINVAL;
     if (win_top < 0 || win_left < 0 || win_top > resize_h - out_h || win_left > resize_w - out_w) return DMLB_EINVAL;
     if ((long long)out_w * C > kResampleMaxRowElems) return DMLB_EINVAL;
-    for (int c = 0; c < C; ++c)
-        if (norm->std[c] == 0.0f) return DMLB_EINVAL;
+    ResampleArgs a;
+    if (!pack_norm(norm, C, a.mean, a.std)) return DMLB_EINVAL;
     if (batch > 0 && (!images || !idx || !boxes || !out)) return DMLB_EINVAL;
     if (((uintptr_t)out & (out_bf16 ? 1 : 3)) != 0 || ((uintptr_t)boxes & 3) != 0) return DMLB_EALIGN;
     if (batch == 0) return DMLB_OK;
 
     const ResamplePlan p = resample_plan(H, W, C, resize_h, resize_w, out_h, out_w);
-    ResampleArgs a;
     a.images = images;
     a.idx = (const long long *)idx;
     a.boxes = boxes;
@@ -804,19 +788,11 @@ int dmlb_image_resample_u8(const uint8_t *images, const int64_t *idx, const int3
     a.H = H, a.W = W, a.C = C, a.rh = resize_h, a.rw = resize_w, a.win_top = win_top, a.win_left = win_left;
     a.oh = out_h, a.ow = out_w;
     a.rows = p.rows, a.bands = p.bands, a.srows = p.srows, a.kx = p.kx, a.ky = p.ky;
-    for (int c = 0; c < 4; ++c) {
-        a.mean[c] = c < C ? norm->mean[c] : 0.0f;
-        a.std[c] = c < C ? norm->std[c] : 1.0f;
-    }
-    const long long jobs = batch * p.bands;
-    const long long cap = (long long)sm_count() * kResampleCtasPerSm;
-    const int grid = (int)(jobs < cap ? jobs : cap);
+    const int grid = band_grid(batch * p.bands, kResampleCtasPerSm);
     cudaStream_t st = (cudaStream_t)stream;
-    if (out_bf16)
-        return channels_last ? launch_resample<true, true>(grid, p.smem, st, a)
-                             : launch_resample<true, false>(grid, p.smem, st, a);
-    return channels_last ? launch_resample<false, true>(grid, p.smem, st, a)
-                         : launch_resample<false, false>(grid, p.smem, st, a);
+    return dispatch_layout(out_bf16, channels_last, [&](auto bf16, auto nhwc) {
+        return launch_resample<decltype(bf16)::value, decltype(nhwc)::value>(grid, p.smem, st, a);
+    });
 }
 
 int dmlb_image_mix(const float *src, const int64_t *idx, const int64_t *labels, const int32_t *erase, const float *fill,

@@ -15,6 +15,26 @@ gather + normalise kernel (libdmlb dmlb_shard_gather_u8) instead of a host DataL
 `DeviceImageDataset` does the same for colour images (HWC uint8) with pad / random or centre crop / horizontal flip /
 per-channel normalisation in one kernel (dmlb_image_batch_u8), and `DeviceResizedImageDataset` does the ImageNet
 recipes (RandomResizedCrop or Resize + CenterCrop, flip, normalise) with one resampling kernel (dmlb_image_resample_u8).
+
+Augmentation draws: the colour-image datasets make every draw here, on the host; the kernels take them as arguments
+or device tables (one per epoch).  They all come from one counter hash:
+  mix(z)     SplitMix64's finaliser: z = (z ^ z >> 30) * 0xbf58476d1ce4e5b9; z = (z ^ z >> 27) * 0x94d049bb133111eb;
+             z ^ z >> 31, in uint64 arithmetic; g = 0x9e3779b97f4a7c15
+  row hash   h = mix(mix(mix(seed + g) ^ (epoch + g)) ^ (row + g)) of a dataset row: a sample's draws depend only on
+             (seed, epoch, row), never on the batch, rank or world size
+  row words  word 0 = h itself, word k = mix(h + k g) for k >= 1; a uniform is u53 = (word >> 11) 2^-53; top and left
+             offsets take top from a word's low and left from its high 32 bits, each as below(u32, n) = u32 n >> 32
+      0        the window of crop_windows (random crops)
+      1        the flip of every dataset: flipped = word 1 >> 63
+      2..31    resized_crop_boxes: attempt a (0..9) takes the area from word 2 + 3a, the log aspect ratio from 3 + 3a,
+               the offsets from 4 + 3a
+      32..62   erase_boxes: erased when u53(word 32) < p; attempt a takes the area from word 33 + 3a, the log aspect
+               ratio from 34 + 3a, the offsets from 35 + 3a
+  batch hash hb = mix(mix(e ^ (rank + g + 2^63)) ^ (batch + g)), e = mix(mix(seed + g) ^ (epoch + g)) (batch_hash); a
+             row's hash is mix(e ^ (row + g)) with row < 2^63 and mix is a bijection, so hb is never a row's hash.
+             mix_batch_params takes the MixUp / CutMix choice from mix(hb + g) >> 63, CutMix's centre from
+             mix(hb + 2 g) and lam ~ Beta(alpha, alpha) from Marsaglia-Tsang Gamma draws on the (0, 1] uniforms
+             ((mix(hb + k g) >> 11) + 1) 2^-53, k = 3, 4, ...
 """
 import ctypes
 import math
@@ -275,64 +295,36 @@ class DeviceShardedDataset:
             yield x, y
 
 
-class DeviceImageDataset(DeviceShardedDataset):
-    """Device-resident colour-image dataset with the usual training augmentation (SURVEY §8f-1).
+def _image_hwc(images):
+    """(H, W, C) of uint8 [N, H, W, C] images; anything else is refused."""
+    if images.dim() != 4 or not 1 <= images.shape[3] <= 4:
+        raise ValueError('images must be uint8 [N, H, W, C] with 1 <= C <= 4')
+    return tuple(int(v) for v in images.shape[1:])
 
-    images: uint8 [N, H, W, C] (HWC, C <= 4), labels: int64 [N].  Each batch is one libdmlb launch
-    (dmlb_image_batch_u8) plus the label gather, and equals, bit for bit, torchvision's
-        pad(padding, fill=0) -> crop (random or centre) -> hflip (probability 1/2) -> to_tensor -> normalize(mean, std)
-    on every sample.  x is [B, C, h, w] in `memory_format` (torch.contiguous_format or torch.channels_last), in
-    `out_dtype` (float32 or bfloat16).  crop: None (the whole padded image), an int or (h, w).  random_crop=False takes
-    the centre window (validation).  A sample's window and flip depend only on (aug_seed, epoch, its dataset index), so
-    they are the same at every rank and world size; set_epoch advances the shard permutation and the augmentation
-    together.  Sharding, shuffle, even_shards and drop_last are DeviceShardedDataset's.
 
-    Batch mixing (torchvision v2's classification recipe after Normalize; every argument off by default):
-      random_erase  RandomErasing(p=random_erase, scale=erase_scale, ratio=erase_ratio, value=erase_value) on every
-                    sample; value is a number or one per channel ('random' is refused).  The boxes depend only on
-                    (aug_seed, epoch, dataset index), like the crops (erase_boxes).
-      mixup_alpha, cutmix_alpha   RandomChoice([MixUp(mixup_alpha), CutMix(cutmix_alpha)]) on every batch (only the one
-                    whose alpha is > 0 when the other is 0), with num_classes one-hot targets.  The choice and the draws
-                    depend on (aug_seed, epoch, rank, batch number): batches are rank-local, so unlike the crops these
-                    differ between ranks and world sizes (mix_batch_params).
-    With either alpha > 0 the batches are (x, targets), targets fp32 [B, num_classes] (label smoothing belongs to the
-    loss, as in torchvision); with erasing alone they are (x, int64 y).  Either way each batch is two launches: the image
-    kernel writes an fp32 scratch batch and dmlb_image_mix erases, mixes and writes x and the targets.
-    mix_params() gives the erase table and the per-batch draws of the epoch.
-    """
+class _DeviceImageBatches(DeviceShardedDataset):
+    """What the colour-image datasets share: normalisation, layout, batch mixing and the batch loop.  A subclass checks
+    its geometry, passes its output size `crop` and supplies epoch_table() (numpy int32, one row per sample of this
+    rank's epoch, in iteration order) and _launch(view, table_rows, x), which writes the images of `view` into x."""
 
-    def __init__(self, images, labels, batch_size, mean, std, crop=None, padding=0, random_crop=True, hflip=False,
-                 memory_format=torch.contiguous_format, out_dtype=torch.float32, shuffle=True, even_shards=True, seed=0,
-                 aug_seed=None, rank=None, world_size=None, device=None, drop_last=False, mixup_alpha=0.0,
-                 cutmix_alpha=0.0, num_classes=None, random_erase=0.0, erase_scale=(0.02, 0.33), erase_ratio=(0.3, 3.3),
-                 erase_value=0.0):
-        if images.dim() != 4 or not 1 <= images.shape[3] <= 4:
-            raise ValueError('images must be uint8 [N, H, W, C] with 1 <= C <= 4')
+    def __init__(self, images, labels, batch_size, mean, std, crop, hflip, memory_format, out_dtype, shuffle,
+                 even_shards, seed, aug_seed, rank, world_size, device, drop_last, mixup_alpha, cutmix_alpha,
+                 num_classes, random_erase, erase_scale, erase_ratio, erase_value):
         if memory_format not in (torch.contiguous_format, torch.channels_last):
             raise ValueError('memory_format must be torch.contiguous_format or torch.channels_last')
         super().__init__(images, labels, batch_size, shuffle=shuffle, even_shards=even_shards, seed=seed, rank=rank,
                          world_size=world_size, device=device, out_dtype=out_dtype, drop_last=drop_last)
-        H, W, C = self.item_shape
+        C = self.item_shape[2]
         mean, std = [float(m) for m in mean], [float(s) for s in std]
         if len(mean) != C or len(std) != C:
             raise ValueError(f'mean and std need one value per channel ({C})')
         if any(s == 0.0 for s in std):
             raise ValueError('std must not be 0')
         self.mean, self.std = mean, std
-        self.padding = int(padding)
-        if crop is None:
-            crop = (H + 2 * self.padding, W + 2 * self.padding)
-        self.crop = (int(crop), int(crop)) if isinstance(crop, int) else tuple(int(c) for c in crop)
-        if self.padding < 0 or not (0 < self.crop[0] <= H + 2 * self.padding and 0 < self.crop[1] <= W + 2 * self.padding):
-            raise ValueError(f'crop {self.crop} does not fit the {H}x{W} images padded by {self.padding}')
-        self.random_crop, self.hflip = bool(random_crop), bool(hflip)
+        self.crop, self.hflip = crop, bool(hflip)
         self.memory_format = memory_format
         self.aug_seed = seed if aug_seed is None else aug_seed
         self._norm = self._N.ImageNorm.of(mean, std)
-        self._init_mixing(mixup_alpha, cutmix_alpha, num_classes, random_erase, erase_scale, erase_ratio, erase_value)
-
-    def _init_mixing(self, mixup_alpha, cutmix_alpha, num_classes, random_erase, erase_scale, erase_ratio, erase_value):
-        C = self.item_shape[2]
         self.mixup_alpha, self.cutmix_alpha = float(mixup_alpha), float(cutmix_alpha)
         if not (self.mixup_alpha >= 0.0 and self.cutmix_alpha >= 0.0):
             raise ValueError(f'mixup_alpha and cutmix_alpha must be >= 0, got {mixup_alpha}, {cutmix_alpha}')
@@ -386,6 +378,19 @@ class DeviceImageDataset(DeviceShardedDataset):
         return (self.epoch_indices(), torch.from_numpy(self.epoch_erase_boxes()).to(self.device),
                 [self.batch_params(n) for n in range(len(self))])
 
+    def augment_params(self):
+        """(indices, table): this rank's dataset indices for the current epoch in iteration order, and the device copy
+        of epoch_table(), as the batches of this epoch use them."""
+        return self.epoch_indices(), torch.from_numpy(self.epoch_table()).to(self.device)
+
+    def _empty(self, b, dtype=None):
+        C = self.item_shape[2]
+        h, w = self.crop
+        dtype = self.out_dtype if dtype is None else dtype
+        if self.memory_format == torch.channels_last:
+            return torch.empty((b, h, w, C), dtype=dtype, device=self.device).permute(0, 3, 1, 2)
+        return torch.empty((b, C, h, w), dtype=dtype, device=self.device)
+
     def _mixed(self, view, scratch, erase, batch):
         """Erase, mix and write the batch of the rows `view` from its fp32 `scratch` (one dmlb_image_mix launch)."""
         N = self._N
@@ -406,73 +411,101 @@ class DeviceImageDataset(DeviceShardedDataset):
             N.stream_ptr()), 'image_mix')
         return x, y
 
-    def _batches(self, idx, launch):
-        """The epoch's batches of the rows `idx`: launch(start, view, x) writes the images of idx[start:start + len(view)]
-        into x, then the labels are gathered, or (batch mixing) x is an fp32 scratch batch that dmlb_image_mix erases
-        and mixes into the yielded batch together with its targets."""
+    def __iter__(self):
+        """The epoch's batches: _launch writes the images of each batch into x, then the labels are gathered, or (batch
+        mixing) x is an fp32 scratch batch that dmlb_image_mix erases and mixes into the yielded batch together with
+        its targets."""
         N = self._N
         lib = N.cuda_lib(self.device.index)
+        idx, table = self.augment_params()
         count = idx.numel()
         erase = None
-        if self._mixing and self.random_erase > 0.0:
+        if self.random_erase > 0.0:
             erase = torch.from_numpy(self.epoch_erase_boxes()).to(self.device)
         for start in range(0, count, self.batch_size):
             b = min(self.batch_size, count - start)
             if b < self.batch_size and self.drop_last:
                 return
-            view = idx[start:start + b]
+            view, rows = idx[start:start + b], table[start:start + b]
             if self._mixing:
                 scratch = self._empty(b, torch.float32)
-                launch(start, view, scratch)
+                self._launch(view, rows, scratch)
                 yield self._mixed(view, scratch, None if erase is None else erase[start:start + b],
                                   start // self.batch_size)
                 continue
             x = self._empty(b)
             y = torch.empty(b, dtype=torch.int64, device=self.device)
-            launch(start, view, x)
+            self._launch(view, rows, x)
             N.check(lib.dmlb_shard_gather_i64(self.labels.data_ptr(), view.data_ptr(), b, y.data_ptr(), N.stream_ptr()),
                     'shard_gather_i64')
             yield x, y
 
-    def _launch(self, idx, x, params=None):
+
+class DeviceImageDataset(_DeviceImageBatches):
+    """Device-resident colour-image dataset with the usual training augmentation (SURVEY §8f-1).
+
+    images: uint8 [N, H, W, C] (HWC, C <= 4), labels: int64 [N].  Each batch is one libdmlb launch
+    (dmlb_image_batch_u8) plus the label gather, and equals, bit for bit, torchvision's
+        pad(padding, fill=0) -> crop (random or centre) -> hflip (probability 1/2) -> to_tensor -> normalize(mean, std)
+    on every sample.  x is [B, C, h, w] in `memory_format` (torch.contiguous_format or torch.channels_last), in
+    `out_dtype` (float32 or bfloat16).  crop: None (the whole padded image), an int or (h, w).  random_crop=False takes
+    the centre window (validation).  A sample's window and flip depend only on (aug_seed, epoch, its dataset index), so
+    they are the same at every rank and world size (crop_windows, drawn on the host and uploaded once per epoch);
+    set_epoch advances the shard permutation and the augmentation together.  Sharding, shuffle, even_shards and
+    drop_last are DeviceShardedDataset's.  augment_params() gives the epoch's indices and windows.
+
+    Batch mixing (torchvision v2's classification recipe after Normalize; every argument off by default):
+      random_erase  RandomErasing(p=random_erase, scale=erase_scale, ratio=erase_ratio, value=erase_value) on every
+                    sample; value is a number or one per channel ('random' is refused).  The boxes depend only on
+                    (aug_seed, epoch, dataset index), like the crops (erase_boxes).
+      mixup_alpha, cutmix_alpha   RandomChoice([MixUp(mixup_alpha), CutMix(cutmix_alpha)]) on every batch (only the one
+                    whose alpha is > 0 when the other is 0), with num_classes one-hot targets.  The choice and the draws
+                    depend on (aug_seed, epoch, rank, batch number): batches are rank-local, so unlike the crops these
+                    differ between ranks and world sizes (mix_batch_params).
+    With either alpha > 0 the batches are (x, targets), targets fp32 [B, num_classes] (label smoothing belongs to the
+    loss, as in torchvision); with erasing alone they are (x, int64 y).  Either way each batch is two launches: the image
+    kernel writes an fp32 scratch batch and dmlb_image_mix erases, mixes and writes x and the targets.
+    mix_params() gives the erase table and the per-batch draws of the epoch.
+    """
+
+    def __init__(self, images, labels, batch_size, mean, std, crop=None, padding=0, random_crop=True, hflip=False,
+                 memory_format=torch.contiguous_format, out_dtype=torch.float32, shuffle=True, even_shards=True, seed=0,
+                 aug_seed=None, rank=None, world_size=None, device=None, drop_last=False, mixup_alpha=0.0,
+                 cutmix_alpha=0.0, num_classes=None, random_erase=0.0, erase_scale=(0.02, 0.33), erase_ratio=(0.3, 3.3),
+                 erase_value=0.0):
+        H, W, _ = _image_hwc(images)
+        self.padding = int(padding)
+        if crop is None:
+            crop = (H + 2 * self.padding, W + 2 * self.padding)
+        crop = (int(crop), int(crop)) if isinstance(crop, int) else tuple(int(c) for c in crop)
+        if self.padding < 0 or not (0 < crop[0] <= H + 2 * self.padding and 0 < crop[1] <= W + 2 * self.padding):
+            raise ValueError(f'crop {crop} does not fit the {H}x{W} images padded by {self.padding}')
+        self.random_crop = bool(random_crop)
+        super().__init__(images, labels, batch_size, mean, std, crop, hflip, memory_format, out_dtype, shuffle,
+                         even_shards, seed, aug_seed, rank, world_size, device, drop_last, mixup_alpha, cutmix_alpha,
+                         num_classes, random_erase, erase_scale, erase_ratio, erase_value)
+
+    def epoch_table(self):
+        """int32 [shard_len(), 3] numpy {top, left, flipped} (crop_windows) of this rank's samples this epoch, in
+        iteration order."""
+        H, W, _ = self.item_shape
+        return crop_windows(self._shard_rows(), H, W, *self.crop, self.padding, self.random_crop, self.hflip,
+                            self.aug_seed, self.epoch)
+
+    def _launch(self, view, windows, x):
         N = self._N
         H, W, C = self.item_shape
-        lib = N.cuda_lib(self.device.index)
-        N.check(lib.dmlb_image_batch_u8(self.images.data_ptr(), idx.data_ptr(), idx.numel(), H, W, C, self.crop[0],
-                                        self.crop[1], self.padding, int(self.random_crop), int(self.hflip),
-                                        self.aug_seed % (1 << 64), self.epoch, self._norm, x.data_ptr(),
-                                        int(x.dtype == torch.bfloat16),
-                                        int(self.memory_format == torch.channels_last),
-                                        None if params is None else params.data_ptr(), N.stream_ptr()),
-                'image_batch_u8')
-
-    def _empty(self, b, dtype=None):
-        C = self.item_shape[2]
-        h, w = self.crop
-        dtype = self.out_dtype if dtype is None else dtype
-        if self.memory_format == torch.channels_last:
-            return torch.empty((b, h, w, C), dtype=dtype, device=self.device).permute(0, 3, 1, 2)
-        return torch.empty((b, C, h, w), dtype=dtype, device=self.device)
-
-    def augment_params(self):
-        """(indices, params): this rank's dataset indices for the current epoch in iteration order, and the int32
-        [count, 3] {top, left, flipped} of each (top/left in padded coordinates), as the batches of this epoch use them."""
-        idx = self.epoch_indices()
-        params = torch.empty((idx.numel(), 3), dtype=torch.int32, device=self.device)
-        for start in range(0, idx.numel(), self.batch_size):
-            view = idx[start:start + self.batch_size]
-            self._launch(view, self._empty(view.numel()), params[start:start + view.numel()])
-        return idx, params
-
-    def __iter__(self):
-        yield from self._batches(self.epoch_indices(), lambda start, view, x: self._launch(view, x))
+        N.check(N.cuda_lib(self.device.index).dmlb_image_batch_u8(
+            self.images.data_ptr(), view.data_ptr(), windows.data_ptr(), view.numel(), H, W, C, *self.crop,
+            self.padding, self._norm, x.data_ptr(), int(x.dtype == torch.bfloat16),
+            int(self.memory_format == torch.channels_last), N.stream_ptr()), 'image_batch_u8')
 
 
 _GAMMA = np.uint64(0x9E3779B97F4A7C15)
 
 
 def _mix(z):
-    """SplitMix64's finaliser on uint64 arrays (the hash of dmlb_image_batch_u8, include/dmlb.h)."""
+    """SplitMix64's finaliser on uint64 arrays."""
     with np.errstate(over='ignore'):
         z = (z ^ (z >> np.uint64(30))) * np.uint64(0xBF58476D1CE4E5B9)
         z = (z ^ (z >> np.uint64(27))) * np.uint64(0x94D049BB133111EB)
@@ -487,93 +520,95 @@ def _row_hash(rows, seed, epoch):
         return _mix(h ^ (np.asarray(rows, dtype=np.int64).astype(np.uint64) + _GAMMA))
 
 
+def _word(h, k):
+    """Row word k >= 1 of the row hashes h: mix(h + k g)."""
+    with np.errstate(over='ignore'):
+        return _mix(h + np.uint64(k) * _GAMMA)
+
+
+def _u53(h, k):
+    """The uniform [0, 1) of row word k: its top 53 bits * 2^-53."""
+    return (_word(h, k) >> np.uint64(11)).astype(np.float64) * 2.0 ** -53
+
+
 def _below(u32, n):
     """u32 * n >> 32: a uniform 32-bit word mapped onto [0, n)."""
-    with np.errstate(over='ignore'):
-        return ((u32 * np.asarray(n).astype(np.uint64)) >> np.uint64(32)).astype(np.int64)
+    return ((u32 * np.asarray(n).astype(np.uint64)) >> np.uint64(32)).astype(np.int64)
+
+
+def _flips(h, hflip):
+    """flipped = word 1 >> 63 of every row hash when hflip, else 0 (int64)."""
+    if not hflip:
+        return np.zeros(len(h), dtype=np.int64)
+    return (_word(h, 1) >> np.uint64(63)).astype(np.int64)
+
+
+def crop_windows(rows, H, W, out_h, out_w, pad, random_crop, hflip, seed, epoch):
+    """int32 [len(rows), 3] {top, left, flipped}, top / left in padded coordinates: the out_h x out_w window of every
+    row's H x W image padded by `pad`, random (top and left from row word 0, the hash itself) or centred (round(d / 2),
+    halves to even, as torchvision center_crop), flipped from row word 1 when hflip.  Vectorised over the rows."""
+    h = _row_hash(rows, seed, epoch)
+    dy, dx = H + 2 * pad - out_h, W + 2 * pad - out_w
+    if random_crop:
+        top, left = _below(h & np.uint64(0xFFFFFFFF), dy + 1), _below(h >> np.uint64(32), dx + 1)
+    else:
+        top, left = np.full(len(h), round(dy / 2)), np.full(len(h), round(dx / 2))
+    return np.stack([top, left, _flips(h, hflip)], axis=-1).astype(np.int32)
 
 
 def resized_crop_boxes(rows, H, W, scale, ratio, seed, epoch, hflip):
     """int32 [len(rows), 5] {top, left, height, width, flipped}: torchvision RandomResizedCrop.get_params for every
-    row, its uniform draws taken from the counter hash h = mix(mix(mix(seed + g) ^ (epoch + g)) ^ (row + g)), so a box
-    depends only on (seed, epoch, row).  Attempt a (0..9) takes the area fraction from the 53-bit uniform of
-    mix(h + (2 + 3a) g), the log aspect ratio from mix(h + (3 + 3a) g) and the offsets from mix(h + (4 + 3a) g) (top from
-    its low, left from its high 32 bits, u32 * n >> 32); w and h round halves to even; after 10 failed attempts the box
-    is torchvision's central fallback.  flipped = mix(h + g) >> 63 when hflip.  fp64 numpy, vectorised over the rows."""
-    rows = np.asarray(rows, dtype=np.int64)
-    with np.errstate(over='ignore'):
-        h = _row_hash(rows, seed, epoch)
-
-        def word(k, sel=slice(None)):
-            return _mix(h[sel] + np.uint64(k) * _GAMMA)
-
-        def u53(k):
-            return (word(k) >> np.uint64(11)).astype(np.float64) * 2.0 ** -53
-
-        below = _below
-
-        in_ratio = W / H
-        if in_ratio < min(ratio):
-            fw, fh = W, int(round(W / min(ratio)))
-        elif in_ratio > max(ratio):
-            fh, fw = H, int(round(H * max(ratio)))
-        else:
-            fw, fh = W, H
-        box = np.tile(np.asarray([(H - fh) // 2, (W - fw) // 2, fh, fw], dtype=np.int64), (len(rows), 1))
-        done = np.zeros(len(rows), dtype=bool)
-        lr0, lr1 = np.log(ratio[0]), np.log(ratio[1])
-        for a in range(10):
-            target = H * W * (scale[0] + (scale[1] - scale[0]) * u53(2 + 3 * a))
-            aspect = np.exp(lr0 + (lr1 - lr0) * u53(3 + 3 * a))
-            w = np.rint(np.sqrt(target * aspect)).astype(np.int64)
-            hh = np.rint(np.sqrt(target / aspect)).astype(np.int64)
-            ok = ~done & (w > 0) & (w <= W) & (hh > 0) & (hh <= H)
-            if ok.any():
-                off = word(4 + 3 * a, ok)
-                box[ok] = np.stack([below(off & np.uint64(0xFFFFFFFF), H - hh[ok] + 1),
-                                    below(off >> np.uint64(32), W - w[ok] + 1), hh[ok], w[ok]], axis=-1)
-                done |= ok
-        flip = (_mix(h + _GAMMA) >> np.uint64(63)).astype(np.int64) if hflip else np.zeros(len(rows), dtype=np.int64)
-    return np.concatenate([box, flip[:, None]], axis=1).astype(np.int32)
+    row, drawn from row words 2..31 (and 1 for the flip); w and h round halves to even, and after 10 failed attempts
+    the box is torchvision's central fallback.  fp64 numpy, vectorised over the rows."""
+    h = _row_hash(rows, seed, epoch)
+    in_ratio = W / H
+    if in_ratio < min(ratio):
+        fw, fh = W, int(round(W / min(ratio)))
+    elif in_ratio > max(ratio):
+        fh, fw = H, int(round(H * max(ratio)))
+    else:
+        fw, fh = W, H
+    box = np.tile(np.asarray([(H - fh) // 2, (W - fw) // 2, fh, fw], dtype=np.int64), (len(h), 1))
+    done = np.zeros(len(h), dtype=bool)
+    lr0, lr1 = np.log(ratio[0]), np.log(ratio[1])
+    for a in range(10):
+        target = H * W * (scale[0] + (scale[1] - scale[0]) * _u53(h, 2 + 3 * a))
+        aspect = np.exp(lr0 + (lr1 - lr0) * _u53(h, 3 + 3 * a))
+        w = np.rint(np.sqrt(target * aspect)).astype(np.int64)
+        hh = np.rint(np.sqrt(target / aspect)).astype(np.int64)
+        ok = ~done & (w > 0) & (w <= W) & (hh > 0) & (hh <= H)
+        if ok.any():
+            off = _word(h[ok], 4 + 3 * a)
+            box[ok] = np.stack([_below(off & np.uint64(0xFFFFFFFF), H - hh[ok] + 1),
+                                _below(off >> np.uint64(32), W - w[ok] + 1), hh[ok], w[ok]], axis=-1)
+            done |= ok
+    return np.concatenate([box, _flips(h, hflip)[:, None]], axis=1).astype(np.int32)
 
 
-ERASE_WORD = 32  # the erase words of a row, mix(h + k g) for k in 32..62, follow the crop and flip words (k <= 31)
+ERASE_WORD = 32  # the erase words of a row, 32..62, follow the crop and flip words (0..31)
 
 
 def erase_boxes(rows, h, w, p, scale, ratio, seed, epoch):
     """int32 [len(rows), 5] {top, left, height, width, erased}: torchvision RandomErasing(p, scale, ratio) on an
-    h x w sample for every row, its uniform draws taken from the row's counter hash h_r of resized_crop_boxes, so a box
-    depends only on (seed, epoch, row).  The row is erased when the 53-bit uniform of mix(h_r + 32 g) is below p; then
-    attempt a (0..9) takes the area fraction from mix(h_r + (33 + 3a) g), the log aspect ratio from mix(h_r + (34 + 3a) g)
-    and the offsets from mix(h_r + (35 + 3a) g) (top from its low, left from its high 32 bits, u32 * n >> 32), with
-    make_params' arithmetic: height = round(sqrt(area * aspect)), width = round(sqrt(area / aspect)), halves to even,
-    accepted when height < h and width < w.  After 10 failed attempts, or when not erased, the row is {0, 0, 0, 0, 0}.
-    fp64 numpy, vectorised over the rows."""
-    rows = np.asarray(rows, dtype=np.int64)
-    box = np.zeros((len(rows), 5), dtype=np.int64)
-    with np.errstate(over='ignore'):
-        hr = _row_hash(rows, seed, epoch)
-
-        def word(k, sel=slice(None)):
-            return _mix(hr[sel] + np.uint64(ERASE_WORD + k) * _GAMMA)
-
-        def u53(k):
-            return (word(k) >> np.uint64(11)).astype(np.float64) * 2.0 ** -53
-
-        todo = u53(0) < p
-        lr0, lr1 = np.log(ratio[0]), np.log(ratio[1])
-        for a in range(10):
-            area = h * w * (scale[0] + (scale[1] - scale[0]) * u53(1 + 3 * a))
-            aspect = np.exp(lr0 + (lr1 - lr0) * u53(2 + 3 * a))
-            eh = np.rint(np.sqrt(area * aspect)).astype(np.int64)
-            ew = np.rint(np.sqrt(area / aspect)).astype(np.int64)
-            ok = todo & (eh < h) & (ew < w)
-            if ok.any():
-                off = word(3 + 3 * a, ok)
-                box[ok] = np.stack([_below(off & np.uint64(0xFFFFFFFF), h - eh[ok] + 1),
-                                    _below(off >> np.uint64(32), w - ew[ok] + 1), eh[ok], ew[ok],
-                                    np.ones(int(ok.sum()), dtype=np.int64)], axis=-1)
-                todo &= ~ok
+    h x w sample for every row, drawn from row words 32..62, with make_params' arithmetic: height =
+    round(sqrt(area * aspect)), width = round(sqrt(area / aspect)), halves to even, accepted when height < h and
+    width < w.  After 10 failed attempts, or when not erased, the row is {0, 0, 0, 0, 0}.  fp64 numpy, vectorised."""
+    hr = _row_hash(rows, seed, epoch)
+    box = np.zeros((len(hr), 5), dtype=np.int64)
+    todo = _u53(hr, ERASE_WORD) < p
+    lr0, lr1 = np.log(ratio[0]), np.log(ratio[1])
+    for a in range(10):
+        area = h * w * (scale[0] + (scale[1] - scale[0]) * _u53(hr, ERASE_WORD + 1 + 3 * a))
+        aspect = np.exp(lr0 + (lr1 - lr0) * _u53(hr, ERASE_WORD + 2 + 3 * a))
+        eh = np.rint(np.sqrt(area * aspect)).astype(np.int64)
+        ew = np.rint(np.sqrt(area / aspect)).astype(np.int64)
+        ok = todo & (eh < h) & (ew < w)
+        if ok.any():
+            off = _word(hr[ok], ERASE_WORD + 3 + 3 * a)
+            box[ok] = np.stack([_below(off & np.uint64(0xFFFFFFFF), h - eh[ok] + 1),
+                                _below(off >> np.uint64(32), w - ew[ok] + 1), eh[ok], ew[ok],
+                                np.ones(int(ok.sum()), dtype=np.int64)], axis=-1)
+            todo &= ~ok
     return box.astype(np.int32)
 
 
@@ -583,7 +618,7 @@ MIXUP, CUTMIX = 1, 2
 
 
 def _mix_int(z):
-    """_mix on one python int."""
+    """_mix on one python int: 4x faster than numpy scalars on the per-batch draws."""
     z &= _M64
     z = ((z ^ (z >> 30)) * 0xBF58476D1CE4E5B9) & _M64
     z = ((z ^ (z >> 27)) * 0x94D049BB133111EB) & _M64
@@ -591,8 +626,7 @@ def _mix_int(z):
 
 
 def batch_hash(seed, epoch, rank, batch):
-    """hb = mix(mix(e ^ (rank + g + 2^63)) ^ (batch + g)), e = mix(mix(seed + g) ^ (epoch + g)).  A row's hash is
-    mix(e ^ (row + g)) with row < 2^63, and mix is a bijection, so no rank's word is ever a row's."""
+    """hb = mix(mix(e ^ (rank + g + 2^63)) ^ (batch + g)), e = mix(mix(seed + g) ^ (epoch + g)): never a row's hash."""
     e = _mix_int(_mix_int(seed + _G) ^ ((epoch + _G) & _M64))
     return _mix_int(_mix_int(e ^ ((rank + _G + (1 << 63)) & _M64)) ^ ((batch + _G) & _M64))
 
@@ -633,11 +667,10 @@ def cutmix_box(lam, r_x, r_y, h, w):
 
 def mix_batch_params(seed, epoch, rank, batch, h, w, mixup_alpha, cutmix_alpha):
     """{'mode', 'lam', 'lam_adjusted', 'box'} of batch number `batch` of `rank` in `epoch`: torchvision
-    RandomChoice([MixUp(mixup_alpha), CutMix(cutmix_alpha)]) on an h x w batch, its draws taken from the words
-    mix(hb + k g) of batch_hash (the batches are rank-local, so these draws depend on the rank).
-      mode   MIXUP or CUTMIX when only that alpha is > 0; with both, MIXUP + (mix(hb + g) >> 63); 0 when neither is
-      lam    Beta(alpha, alpha) of the chosen mode (beta_sample), its (0, 1] uniforms ((mix(hb + k g) >> 11) + 1) 2^-53
-             for k = 3, 4, ...
+    RandomChoice([MixUp(mixup_alpha), CutMix(cutmix_alpha)]) on an h x w batch, drawn from the words mix(hb + k g) of
+    batch_hash (the batches are rank-local, so these draws depend on the rank).
+      mode   MIXUP or CUTMIX when only that alpha is > 0, a choice between them when both are; 0 when neither is
+      lam    Beta(alpha, alpha) of the chosen mode (beta_sample)
       box    CutMix's (x1, y1, x2, y2) (cutmix_box) for r_x = lo32(w2) * w >> 32, r_y = hi32(w2) * h >> 32,
              w2 = mix(hb + 2 g); (0, 0, 0, 0) for MixUp
       lam_adjusted   the weight of the targets: CutMix's lam_adjusted, MixUp's lam."""
@@ -667,7 +700,7 @@ def mix_batch_params(seed, epoch, rank, batch, h, w, mixup_alpha, cutmix_alpha):
     return {'mode': mode, 'lam': lam, 'lam_adjusted': lam_adjusted, 'box': box}
 
 
-class DeviceResizedImageDataset(DeviceImageDataset):
+class DeviceResizedImageDataset(_DeviceImageBatches):
     """Device-resident colour-image dataset with the ImageNet recipes (SURVEY §8f-1), one resampling launch per batch
     (dmlb_image_resample_u8) plus the label gather.
 
@@ -680,7 +713,8 @@ class DeviceResizedImageDataset(DeviceImageDataset):
     they are the same at every rank and world size.  Sharding, shuffle, even_shards and drop_last are
     DeviceShardedDataset's.  The kernel takes image and resized sides of at most 32768, resizes at
     most 8x down on each axis and writes rows of at most 1024 values; the constructor refuses anything else.
-    Batch mixing (random_erase, mixup_alpha, cutmix_alpha, ...) is DeviceImageDataset's, on the size[0] x size[1] output.
+    augment_params() gives the epoch's indices and boxes.  Batch mixing (random_erase, mixup_alpha, cutmix_alpha, ...)
+    is DeviceImageDataset's, on the size[0] x size[1] output.
     """
 
     def __init__(self, images, labels, batch_size, mean, std, size, scale=(0.08, 1.0), ratio=(3 / 4, 4 / 3),
@@ -688,17 +722,11 @@ class DeviceResizedImageDataset(DeviceImageDataset):
                  out_dtype=torch.float32, shuffle=True, even_shards=True, seed=0, aug_seed=None, rank=None,
                  world_size=None, device=None, drop_last=False, mixup_alpha=0.0, cutmix_alpha=0.0, num_classes=None,
                  random_erase=0.0, erase_scale=(0.02, 0.33), erase_ratio=(0.3, 3.3), erase_value=0.0):
-        super().__init__(images, labels, batch_size, mean, std, crop=None, padding=0, random_crop=random, hflip=hflip,
-                         memory_format=memory_format, out_dtype=out_dtype, shuffle=shuffle, even_shards=even_shards,
-                         seed=seed, aug_seed=aug_seed, rank=rank, world_size=world_size, device=device,
-                         drop_last=drop_last, mixup_alpha=mixup_alpha, cutmix_alpha=cutmix_alpha,
-                         num_classes=num_classes, random_erase=random_erase, erase_scale=erase_scale,
-                         erase_ratio=erase_ratio, erase_value=erase_value)
-        H, W, C = self.item_shape
+        H, W, C = _image_hwc(images)
         size = (int(size), int(size)) if isinstance(size, (int, np.integer)) else tuple(int(v) for v in size)
         if len(size) != 2 or min(size) < 1:
             raise ValueError(f'size must be a positive int or (h, w), got {size}')
-        self.crop = size
+        self.random = bool(random)
         self.scale, self.ratio = tuple(float(v) for v in scale), tuple(float(v) for v in ratio)
         if random:
             if not 0.0 < self.scale[0] <= self.scale[1] <= 1.0:
@@ -723,35 +751,25 @@ class DeviceResizedImageDataset(DeviceImageDataset):
             raise ValueError(f'{H}x{W} images resized to {self.resized} is more than an 8x downscale')
         if size[1] * C > 1024:
             raise ValueError(f'size[1] * C = {size[1] * C} is above the 1024 values per output row the kernel takes')
+        super().__init__(images, labels, batch_size, mean, std, size, hflip, memory_format, out_dtype, shuffle,
+                         even_shards, seed, aug_seed, rank, world_size, device, drop_last, mixup_alpha, cutmix_alpha,
+                         num_classes, random_erase, erase_scale, erase_ratio, erase_value)
 
-    def epoch_boxes(self):
+    def epoch_table(self):
         """int32 [shard_len(), 5] numpy {top, left, height, width, flipped} of this rank's samples this epoch, in
-        iteration order."""
+        iteration order: resized_crop_boxes, or the whole image with the same flips in validation."""
         H, W, _ = self.item_shape
         rows = self._shard_rows()
-        if self.random_crop:
+        if self.random:
             return resized_crop_boxes(rows, H, W, self.scale, self.ratio, self.aug_seed, self.epoch, self.hflip)
         boxes = np.tile(np.asarray([0, 0, H, W, 0], dtype=np.int32), (len(rows), 1))
-        if self.hflip:
-            boxes[:, 4] = resized_crop_boxes(rows, H, W, self.scale, self.ratio, self.aug_seed, self.epoch, True)[:, 4]
+        boxes[:, 4] = _flips(_row_hash(rows, self.aug_seed, self.epoch), self.hflip)
         return boxes
 
-    def _launch(self, idx, x, boxes):
+    def _launch(self, view, boxes, x):
         N = self._N
         H, W, C = self.item_shape
-        lib = N.cuda_lib(self.device.index)
-        N.check(lib.dmlb_image_resample_u8(self.images.data_ptr(), idx.data_ptr(), boxes.data_ptr(), idx.numel(), H, W,
-                                           C, self.resized[0], self.resized[1], self.window[0], self.window[1],
-                                           self.crop[0], self.crop[1], self._norm, x.data_ptr(),
-                                           int(x.dtype == torch.bfloat16),
-                                           int(self.memory_format == torch.channels_last), N.stream_ptr()),
-                'image_resample_u8')
-
-    def augment_params(self):
-        """(indices, boxes): this rank's dataset indices for the current epoch in iteration order, and the device int32
-        [count, 5] {top, left, height, width, flipped} the batches of this epoch use."""
-        return self.epoch_indices(), torch.from_numpy(self.epoch_boxes()).to(self.device)
-
-    def __iter__(self):
-        idx, boxes = self.augment_params()
-        yield from self._batches(idx, lambda start, view, x: self._launch(view, x, boxes[start:start + view.numel()]))
+        N.check(N.cuda_lib(self.device.index).dmlb_image_resample_u8(
+            self.images.data_ptr(), view.data_ptr(), boxes.data_ptr(), view.numel(), H, W, C, *self.resized,
+            *self.window, *self.crop, self._norm, x.data_ptr(), int(x.dtype == torch.bfloat16),
+            int(self.memory_format == torch.channels_last), N.stream_ptr()), 'image_resample_u8')

@@ -27,7 +27,7 @@
 extern "C" {
 #endif
 
-#define DMLB_ABI_VERSION 2
+#define DMLB_ABI_VERSION 3
 
 #define DMLB_OK 0
 #define DMLB_EINVAL (-10001)   /* bad argument (null pointer, n out of range, unknown enum)              */
@@ -370,28 +370,22 @@ int dmlb_shard_slice(const int64_t *perm, int64_t first, int64_t count, int64_t 
  *   out[i, c, y, x] = ((float)P[top + y][left + x'][c] / 255.0f - mean[c]) / std[c]   in IEEE fp32, in that order,
  *            P = the image with `pad` zero bytes on all four sides, x' = flipped ? out_w - 1 - x : x
  *            == torchvision pad(fill=0) -> crop -> hflip -> to_tensor -> normalize, bit for bit.
- * The window of a sample depends only on (seed, epoch, row = idx[i]), never on the batch, rank or world size:
- *   mix(z)  = SplitMix64 finaliser: z = (z ^ z >> 30) * 0xbf58476d1ce4e5b9; z = (z ^ z >> 27) * 0x94d049bb133111eb;
- *             z ^ z >> 31   (uint64 arithmetic, g = 0x9e3779b97f4a7c15)
- *   h       = mix(mix(mix(seed + g) ^ (epoch + g)) ^ (row + g))
- *   dy = H + 2 pad - out_h, dx = W + 2 pad - out_w
- *   crop_mode 1 (random): top = ((h & 0xffffffff) * (dy + 1)) >> 32,  left = ((h >> 32) * (dx + 1)) >> 32
- *   crop_mode 0 (centre): top = round(dy / 2), left = round(dx / 2), halves to even (torchvision center_crop)
- *   flipped = hflip ? mix(h + g) >> 63 : 0
- * params_out (optional, DEVICE int32 [batch][3]) receives {top, left, flipped} of every sample.
+ *   windows: DEVICE int32 [batch][3] {top, left, flipped} of every sample, top / left in padded coordinates; the
+ *            datasets sample them on the host (util/data.py crop_windows)
  * DMLB_EINVAL (nothing launched): C outside 1..4, a window larger than the padded image, std[c] == 0 for c < C, a NULL
- * norm, NULL images / idx / out with batch > 0, out_w * C above 49,136 bytes.  DMLB_EALIGN: out not aligned to its
- * element.  Any images alignment works (16-byte loads when images is 16-byte aligned, byte loads otherwise); out is
- * written with 16-byte stores between scalar heads and tails of every contiguous run.
- * Algorithmic bytes/sample: window bytes inside the image read + out_h * out_w * C * (4 | 2) written. */
+ * norm, NULL images / idx / windows / out with batch > 0, out_w * C above 49,136 bytes.  DMLB_EALIGN: out not aligned
+ * to its element or windows not to 4 bytes.  Windows live in device memory and are not checked by the host: a row with
+ * top outside [0, H + 2 pad - out_h] or left outside [0, W + 2 pad - out_w] reads nothing and writes quiet NaN over its
+ * sample; flipped != 0 means flipped.  Any images alignment works (16-byte loads when images is 16-byte aligned, byte
+ * loads otherwise); out is written with 16-byte stores between scalar heads and tails of every contiguous run.
+ * Algorithmic bytes/sample: window bytes inside the image read + out_h * out_w * C * (4 | 2) written + 12 B of window. */
 typedef struct {
     float mean[4];
     float std[4];
 } dmlb_image_norm;
-int dmlb_image_batch_u8(const uint8_t *images, const int64_t *idx, int64_t batch, int32_t H, int32_t W, int32_t C,
-                        int32_t out_h, int32_t out_w, int32_t pad, int crop_mode, int hflip, uint64_t seed, int64_t epoch,
-                        const dmlb_image_norm *norm, void *out, int out_bf16, int channels_last, int32_t *params_out,
-                        void *stream);
+int dmlb_image_batch_u8(const uint8_t *images, const int64_t *idx, const int32_t *windows, int64_t batch, int32_t H,
+                        int32_t W, int32_t C, int32_t out_h, int32_t out_w, int32_t pad, const dmlb_image_norm *norm,
+                        void *out, int out_bf16, int channels_last, void *stream);
 
 /* Resampled colour-image batch: gather + box + antialiased bilinear resize + window + horizontal flip + per-channel
  * normalise, one launch.  torchvision RandomResizedCrop (box per sample, resize = out, window at 0) and
@@ -442,13 +436,7 @@ int dmlb_image_resample_u8(const uint8_t *images, const int64_t *idx, const int3
  *   lam is MixUp's lambda, and CutMix's lam_adjusted = 1 - (x2 - x1)(y2 - y1) / (h w) (both fp64, as python floats);
  *   every multiply and add is rounded once (no FMA), fl32(1 - lam) and fl32(lam) are rounded from fp64 once: torch's
  *   fp32 tensor-by-python-scalar arithmetic, bit for bit.  Label smoothing is left to the loss, as in torchvision.
- * The datasets (util/data.py) sample the arguments on the host from the hash of dmlb_image_batch_u8:
- *   erase rows  per dataset row, h = the row's hash: erased when u53(mix(h + 32 g)) < p; attempt a (0..9) takes the
- *               area fraction from mix(h + (33 + 3a) g), the log aspect from mix(h + (34 + 3a) g), the offsets from
- *               mix(h + (35 + 3a) g) (top low, left high 32 bits) -- words the crop and flip (k <= 31) never use
- *   per batch   hb = mix(mix(e ^ (rank + g + 2^63)) ^ (batch + g)), e = mix(mix(seed + g) ^ (epoch + g)), never a
- *               row's hash; the MixUp / CutMix choice from mix(hb + g) >> 63, CutMix's (r_x, r_y) from mix(hb + 2 g),
- *               lam ~ Beta(alpha, alpha) from Marsaglia-Tsang Gamma draws on the uniforms of mix(hb + k g), k >= 3.
+ * The datasets sample erase, mode, lam and the box on the host (util/data.py erase_boxes, mix_batch_params).
  * Accepted range (anything else: DMLB_EINVAL, nothing launched): C in 1..4; h, w in 1..32768; mode in 0..2;
  * 0 <= lam <= 1; 0 <= y1 <= y2 <= h and 0 <= x1 <= x2 <= w (the box is ignored unless mode == 2); num_classes >= 1
  * when mode != 0; non-NULL src, idx, labels, out and targets when batch > 0, and fill when erase is not NULL.

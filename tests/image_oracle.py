@@ -1,4 +1,5 @@
-"""The colour-image batch rule of dmlb_image_batch_u8 (include/dmlb.h), restated in numpy.
+"""The colour-image batch rule of dmlb_image_batch_u8 (include/dmlb.h) and its window draw (util/data.py), restated
+in numpy.
 
   window   h = mix(mix(mix(seed + g) ^ (epoch + g)) ^ (row + g)), mix = SplitMix64's finaliser, g = 0x9e3779b97f4a7c15
            random: top = (lo32(h) * (dy + 1)) >> 32, left = (hi32(h) * (dx + 1)) >> 32; centre: round(d / 2), halves even

@@ -18,13 +18,13 @@ def declared_symbols():
     return sorted(set(re.findall(r'\b(dmlb_[a-z0-9_]+)\s*\(', text)))
 
 
-def test_library_builds_and_loads_without_gpu():
+def test_library_builds_and_loads_at_abi_version_3_without_gpu():
     from dmlcloud_b200.csrc import build
 
     so = build.build()
     assert so.exists()
     lib = N.load()
-    assert lib.dmlb_abi_version() == N.ABI_VERSION == 2
+    assert lib.dmlb_abi_version() == N.ABI_VERSION == 3
 
 
 def test_header_symbols_are_exported_and_bound():

@@ -1,5 +1,6 @@
 """The colour-image batch rule (dmlb_image_batch_u8, DeviceImageDataset) on the CPU: the numpy oracle equals torchvision
-bit for bit, the window hash has fixed known answers and is uniform, and the C symbol is bound as the header declares it.
+bit for bit, the window hash has fixed known answers and is uniform, the package's window sampler equals the oracle, and
+the C symbol is bound as the header declares it.
 """
 import ctypes
 import re
@@ -103,15 +104,47 @@ def test_hash_known_answers():
         [6, 3, 0], [16, 5, 1], [21, 21, 1], [3, 5, 1]]
 
 
-def test_ctypes_signature_matches_header():
+@pytest.mark.parametrize('case', range(16))
+def test_package_window_sampler_equals_the_oracle(case):
+    """crop_windows against image_oracle.windows over random geometry, both crop modes, flip on and off, and seeds
+    and epochs across the uint64 range."""
+    from dmlcloud_b200.util.data import crop_windows
+
+    rng = np.random.RandomState(200 + case)
+    H, W = (int(v) for v in rng.randint(1, 300, 2))
+    pad = int(rng.randint(0, 9))
+    out_h, out_w = int(rng.randint(1, H + 2 * pad + 1)), int(rng.randint(1, W + 2 * pad + 1))
+    random_crop, hflip = bool(case & 1), bool(case & 2)
+    rows = rng.randint(0, 1 << 40, 2000)
+    for seed in (0, case, 2 ** 63 + case, 2 ** 64 - 1 - case):
+        for epoch in (0, 1 + case, 2 ** 40):
+            got = crop_windows(rows, H, W, out_h, out_w, pad, random_crop, hflip, seed, epoch)
+            assert got.dtype == np.int32 and got.shape == (len(rows), 3)
+            assert (got == O.windows(rows, H, W, out_h, out_w, pad, random_crop, hflip, seed, epoch)).all(), seed
+    assert crop_windows([], H, W, out_h, out_w, pad, random_crop, hflip, 0, 0).shape == (0, 3)
+
+
+def test_windows_are_independent_of_rank_and_world_size():
+    from dmlcloud_b200.util.data import crop_windows
+
+    n = 1001
+    order = np.random.RandomState(3).permutation(n)
+    whole = dict(zip(order.tolist(), map(tuple, crop_windows(order, 37, 41, 29, 33, 2, True, True, 2, 6).tolist())))
+    for world in (2, 3, 8):
+        for rank in range(world):
+            rows = order[rank::world]
+            got = crop_windows(rows, 37, 41, 29, 33, 2, True, True, 2, 6)
+            assert all(whole[r] == tuple(g) for r, g in zip(rows.tolist(), got.tolist()))
+
+
+def test_window_table_signature_matches_header():
     from dmlcloud_b200 import _native as N
 
     text = re.sub(r'/\*.*?\*/', '', (REPO / 'include' / 'dmlb.h').read_text(), flags=re.S)
     decl = re.search(r'int\s+dmlb_image_batch_u8\s*\(([^)]*)\)', text).group(1)
-    ctype = {'const uint8_t*': ctypes.c_void_p, 'const int64_t*': ctypes.c_void_p, 'int64_t': ctypes.c_int64,
-             'int32_t': ctypes.c_int32, 'int': ctypes.c_int, 'uint64_t': ctypes.c_uint64,
-             'const dmlb_image_norm*': ctypes.POINTER(N.ImageNorm), 'void*': ctypes.c_void_p,
-             'int32_t*': ctypes.c_void_p}
+    ctype = {'const uint8_t*': ctypes.c_void_p, 'const int64_t*': ctypes.c_void_p, 'const int32_t*': ctypes.c_void_p,
+             'int64_t': ctypes.c_int64, 'int32_t': ctypes.c_int32, 'int': ctypes.c_int,
+             'const dmlb_image_norm*': ctypes.POINTER(N.ImageNorm), 'void*': ctypes.c_void_p}
     # "const int64_t *idx" -> "const int64_t*": the type with the parameter name dropped
     types = [re.sub(r'\s*\*\s*', '*', re.sub(r'\w+$', '', ' '.join(arg.split())).strip()) for arg in decl.split(',')]
     want = [ctype[t] for t in types]
@@ -121,7 +154,7 @@ def test_ctypes_signature_matches_header():
     assert ctypes.sizeof(N.ImageNorm) == 32 and 'float mean[4];' in text and 'float std[4];' in text
 
 
-def test_invalid_arguments_are_refused_without_a_gpu():
+def test_invalid_arguments_and_window_tables_are_refused_without_a_gpu():
     """Every refusal comes before any CUDA call: fake, aligned device addresses suffice, and nothing is launched."""
     from dmlcloud_b200 import _native as N
 
@@ -130,19 +163,18 @@ def test_invalid_arguments_are_refused_without_a_gpu():
     norm = N.ImageNorm((0.5,) * 4, (0.25,) * 4)
     before = N.launch_count()
 
-    def call(batch=4, H=32, W=32, C=3, oh=32, ow=32, pad=4, mode=1, flip=1, norm=norm, images=a, idx=a, out=a,
-             bf16=0):
-        return lib.dmlb_image_batch_u8(images, idx, batch, H, W, C, oh, ow, pad, mode, flip, 0, 0, norm, out, bf16, 0,
-                                       None, None)
+    def call(batch=4, H=32, W=32, C=3, oh=32, ow=32, pad=4, norm=norm, images=a, idx=a, windows=a, out=a, bf16=0):
+        return lib.dmlb_image_batch_u8(images, idx, windows, batch, H, W, C, oh, ow, pad, norm, out, bf16, 0, None)
 
-    for kw in ({'C': 0}, {'C': 5}, {'oh': 41}, {'ow': 41}, {'pad': 0, 'oh': 33}, {'pad': -1}, {'mode': 2},
-               {'images': None}, {'idx': None}, {'out': None}, {'norm': None}, {'batch': -1}, {'oh': 0},
+    for kw in ({'C': 0}, {'C': 5}, {'oh': 41}, {'ow': 41}, {'pad': 0, 'oh': 33}, {'pad': -1}, {'images': None},
+               {'idx': None}, {'windows': None}, {'out': None}, {'norm': None}, {'batch': -1}, {'oh': 0},
                {'H': 0}, {'W': 64000, 'ow': 16384, 'C': 4, 'pad': 0}):
         assert call(**kw) == N.EINVAL, kw
     zero_std = N.ImageNorm((0.5,) * 4, (0.25, 0.25, 0.0, 0.25))
     assert call(norm=zero_std) == N.EINVAL
     assert call(out=ctypes.c_void_p(258)) == N.EALIGN       # fp32 output off its 4-byte grid
-    assert call(batch=0, images=None, idx=None, out=None) == N.OK
+    assert call(windows=ctypes.c_void_p(258)) == N.EALIGN   # the window table off its 4-byte grid
+    assert call(batch=0, images=None, idx=None, windows=None, out=None) == N.OK
     assert N.launch_count() == before
 
 

@@ -1,6 +1,7 @@
 """dmlb_image_batch_u8 / DeviceImageDataset on the GPU: bit-exact against tests/image_oracle.py (itself pinned against
 torchvision in tests/test_device_images.py) for every layout, dtype, crop mode and alignment; the launch structure; the
-refusals; reproducibility and rank independence of the augmentation; and training runs fed by it."""
+refusals and out-of-range windows; reproducibility and rank independence of the augmentation; and training runs fed by
+it."""
 import functools
 import json
 from pathlib import Path
@@ -48,16 +49,23 @@ def dataset(shape, n, seed):
     return images, mean, std
 
 
+def oracle_windows(idx_dev, shape, random_crop, hflip, seed=3, epoch=1):
+    """The device int32 [b][3] window table image_oracle.windows gives the rows idx_dev."""
+    H, W, C, oh, ow, pad = SHAPES[shape]
+    return torch.from_numpy(O.windows(idx_dev.cpu().numpy(), H, W, oh, ow, pad, random_crop, hflip, seed, epoch)).cuda()
+
+
 def launch(images_dev, idx_dev, shape, mean, std, random_crop, hflip, bf16, channels_last, seed=3, epoch=1, out=None,
-           params=None):
+           windows=None):
+    """One dmlb_image_batch_u8 call on the oracle's windows of the rows idx_dev, or on `windows` when given."""
     N = N_()
     H, W, C, oh, ow, pad = SHAPES[shape]
-    b = idx_dev.numel()
+    if windows is None:
+        windows = oracle_windows(idx_dev, shape, random_crop, hflip, seed, epoch)
     norm = N.ImageNorm.of(mean, std)
-    return N.cuda_lib(0).dmlb_image_batch_u8(images_dev.data_ptr(), idx_dev.data_ptr(), b, H, W, C, oh, ow, pad,
-                                             int(random_crop), int(hflip), seed, epoch, norm, out.data_ptr(), int(bf16),
-                                             int(channels_last), None if params is None else params.data_ptr(),
-                                             N.stream_ptr())
+    return N.cuda_lib(0).dmlb_image_batch_u8(images_dev.data_ptr(), idx_dev.data_ptr(), windows.data_ptr(),
+                                             idx_dev.numel(), H, W, C, oh, ow, pad, norm, out.data_ptr(), int(bf16),
+                                             int(channels_last), N.stream_ptr())
 
 
 def flat_out(shape, b, bf16, offset=0):
@@ -87,7 +95,7 @@ def assert_same_bits(got, want_):
 @pytest.mark.parametrize('hflip', [False, True], ids=['noflip', 'flip'])
 @pytest.mark.parametrize('random_crop', [False, True], ids=['centre', 'random'])
 @pytest.mark.parametrize('shape', list(SHAPES))
-def test_kernel_is_bit_exact_with_the_oracle(shape, random_crop, hflip, bf16, channels_last):
+def test_kernel_is_bit_exact_on_the_oracle_windows(shape, random_crop, hflip, bf16, channels_last):
     """Batch 1, a short batch, and a batch with more band jobs than the capped grid has CTAs (each CTA walks several)."""
     H, W, C, oh, ow, pad = SHAPES[shape]
     bands, _ = geometry(H, W, C, oh, ow, pad, 1)
@@ -102,17 +110,13 @@ def test_kernel_is_bit_exact_with_the_oracle(shape, random_crop, hflip, bf16, ch
         idx[0] = n - 1  # the last sample of the tensor: its last 16-byte chunk is read without running past the end
         idx_dev = torch.from_numpy(idx).cuda()
         _, out = flat_out(shape, b, bf16)
-        params = torch.full((b, 3), -1, dtype=torch.int32, device='cuda')
-        N_().check(launch(images_dev, idx_dev, shape, mean, std, random_crop, hflip, bf16, channels_last, out=out,
-                          params=params))
-        w, wp = want(images, idx, shape, mean, std, random_crop, hflip, bf16, channels_last)
-        assert_same_bits(out, w)
-        assert (params.cpu().numpy() == wp).all()
+        N_().check(launch(images_dev, idx_dev, shape, mean, std, random_crop, hflip, bf16, channels_last, out=out))
+        assert_same_bits(out, want(images, idx, shape, mean, std, random_crop, hflip, bf16, channels_last)[0])
 
 
 @pytest.mark.parametrize('bf16', [False, True], ids=['fp32', 'bf16'])
 @pytest.mark.parametrize('shape', list(SHAPES))
-def test_misaligned_images_and_outputs(shape, bf16):
+def test_misaligned_images_and_outputs_on_the_oracle_windows(shape, bf16):
     """images one byte off 16-byte alignment (byte-load path) and out one element off (scalar heads / tails)."""
     H, W, C, oh, ow, pad = SHAPES[shape]
     n = 40
@@ -139,7 +143,7 @@ def test_misaligned_images_and_outputs(shape, bf16):
                                   ('odd_37x41', 5, False, True, True, 0), ('cifar_pad4', 7, True, False, False, 1),
                                   ('imagenet_224', 200, False, True, True, 0)],
                          ids=['cifar_b1', 'imagenet_b64_bf16_nhwc', 'odd_b5', 'cifar_bytes', 'imagenet_capped'])
-def test_launch_structure(case):
+def test_launch_structure_on_a_window_table(case):
     """One launch per call, of the instance the layout / dtype / alignment select, on the grid the host rule gives."""
     shape, b, bf16, channels_last, aligned, img_off = case
     H, W, C, oh, ow, pad = SHAPES[shape]
@@ -149,8 +153,9 @@ def test_launch_structure(case):
     images_dev = raw[img_off:img_off + images.size]
     idx_dev = torch.from_numpy(np.arange(b) % 50).cuda()
     _, out = flat_out(shape, b, bf16)
+    windows = oracle_windows(idx_dev, shape, True, True)
     rc, launches = dmlb_launches(lambda: launch(images_dev, idx_dev, shape, mean, std, True, True, bf16, channels_last,
-                                                out=out))
+                                                out=out, windows=windows))
     N_().check(rc)
     _, grid = geometry(H, W, C, oh, ow, pad, b)
     tf = lambda v: 'true' if v else 'false'  # noqa: E731
@@ -161,30 +166,57 @@ def test_launch_structure(case):
     assert_same_bits(out, want(images, idx_dev.cpu().numpy(), shape, mean, std, True, True, bf16, channels_last)[0])
 
 
-def test_invalid_arguments_launch_nothing():
+def test_invalid_arguments_and_window_tables_launch_nothing():
     N = N_()
     lib = N.cuda_lib(0)
     images = torch.zeros(4 * 32 * 32 * 3, dtype=torch.uint8, device='cuda')
     idx = torch.zeros(4, dtype=torch.int64, device='cuda')
     out = torch.zeros(4 * 3 * 32 * 32, device='cuda')
+    windows = torch.zeros((4, 3), dtype=torch.int32, device='cuda')
     good = N.ImageNorm((0.5,) * 4, (0.25,) * 4)
     torch.cuda.synchronize()
     before = N.launch_count()
 
-    def call(C=3, oh=32, ow=32, pad=4, norm=good, images=images.data_ptr(), out=out.data_ptr()):
-        return lib.dmlb_image_batch_u8(images, idx.data_ptr(), 4, 32, 32, C, oh, ow, pad, 1, 1, 0, 0, norm, out, 0, 0,
-                                       None, N.stream_ptr())
+    def call(C=3, oh=32, ow=32, pad=4, norm=good, images=images.data_ptr(), out=out.data_ptr(),
+             windows=windows.data_ptr()):
+        return lib.dmlb_image_batch_u8(images, idx.data_ptr(), windows, 4, 32, 32, C, oh, ow, pad, norm, out, 0, 0,
+                                       N.stream_ptr())
 
     assert call(C=0) == call(C=5) == N.EINVAL
     assert call(oh=41) == call(ow=41) == call(pad=0, oh=33) == N.EINVAL
     assert call(norm=N.ImageNorm((0.5,) * 4, (0.25, 0.0, 0.25, 0.25))) == N.EINVAL
-    assert call(images=None) == call(out=None) == call(norm=None) == N.EINVAL
-    assert call(out=out.data_ptr() + 2) == N.EALIGN
+    assert call(images=None) == call(out=None) == call(norm=None) == call(windows=None) == N.EINVAL
+    assert call(out=out.data_ptr() + 2) == call(windows=windows.data_ptr() + 2) == N.EALIGN
     torch.cuda.synchronize()
     assert N.launch_count() == before
     assert call(C=3, norm=N.ImageNorm((0.5,) * 4, (0.25, 0.25, 0.25, 0.0))) == N.OK  # channel 3 is not used at C = 3
     torch.cuda.synchronize()
     assert N.launch_count() == before + 1
+
+
+@pytest.mark.parametrize('channels_last', [False, True], ids=['nchw', 'nhwc'])
+@pytest.mark.parametrize('bf16', [False, True], ids=['fp32', 'bf16'])
+def test_a_window_outside_the_padded_image_writes_nan_over_its_sample_only(bf16, channels_last):
+    """Rows whose top or left lies outside [0, dy] x [0, dx] (one past either end, INT32_MIN, INT32_MAX) read nothing
+    and are quiet NaN; every other sample is bit-exact, with any non-zero flipped meaning flipped."""
+    shape = 'odd_37x41'
+    H, W, C, oh, ow, pad = SHAPES[shape]
+    dy, dx = H + 2 * pad - oh, W + 2 * pad - ow
+    images, mean, std = dataset(shape, 40, 15)
+    idx = np.arange(9) * 4 + 3
+    windows = O.windows(idx, H, W, oh, ow, pad, True, True, 3, 1)
+    bad = {1: (dy + 1, 0), 3: (0, -1), 4: (-2 ** 31, 0), 6: (0, 2 ** 31 - 1), 7: (dy, dx + 1), 8: (-1, dx)}
+    for i, (top, left) in bad.items():
+        windows[i, :2] = top, left
+    good = [i for i in range(len(idx)) if i not in bad]
+    windows[good, 2] *= 7
+    _, out = flat_out(shape, len(idx), bf16)
+    N_().check(launch(torch.from_numpy(images).cuda(), torch.from_numpy(idx).cuda(), shape, mean, std, True, True, bf16,
+                      channels_last, out=out, windows=torch.from_numpy(windows).cuda()))
+    raw = out.view(torch.int16 if bf16 else torch.int32).cpu().view(len(idx), -1)
+    assert (raw[sorted(bad)] == (0x7fc0 if bf16 else 0x7fc00000)).all()
+    assert_same_bits(out.view(len(idx), -1)[good], want(images, idx[good], shape, mean, std, True, True, bf16,
+                                                         channels_last)[0])
 
 
 def make_ds(images, labels, **kw):

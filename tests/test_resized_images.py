@@ -91,7 +91,7 @@ def test_box_sampler_known_answers():
         [16, 23, 168, 217, 0], [19, 38, 228, 202, 1], [25, 13, 227, 239, 1], [18, 74, 84, 88, 1]]
     assert R.sample_boxes(range(4), 32, 48, seed=0, epoch=0).tolist() == [
         [3, 21, 29, 27, 1], [0, 15, 24, 29, 1], [3, 22, 17, 22, 1], [15, 23, 17, 21, 0]]
-    # the flip bit is dmlb_image_batch_u8's rule (tests/test_device_images.py pins [0, 1, 1, 1] for these rows)
+    # the flip bit is the window's rule (tests/test_device_images.py pins [0, 1, 1, 1] for these rows)
     assert R.sample_boxes(range(4), 256, 256, seed=1, epoch=5)[:, 4].tolist() == [0, 1, 1, 1]
 
 
