@@ -135,6 +135,8 @@ SIGNATURES = {
     'dmlb_image_mix': (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, POINTER(c_float), c_int64, c_int32, c_int32,
                                c_int32, c_int, c_double, c_int32, c_int32, c_int32, c_int32, c_int32, c_void_p, c_int,
                                c_int, c_void_p, c_void_p]),
+    'dmlb_image_trivial_augment': (c_int, [c_void_p, c_void_p, c_int64, c_int32, c_int32, c_int32, c_int,
+                                           POINTER(ImageNorm), c_void_p, c_int, c_int, c_void_p]),
 }
 
 _lib = None

@@ -9,6 +9,8 @@
 #include <cmath>
 #include <type_traits>
 
+#include <cooperative_groups.h>
+
 #include "dmlb_common.cuh"
 
 namespace dmlb {
@@ -680,6 +682,325 @@ static int launch_mix(dim3 grid, cudaStream_t st, const MixArgs &a) {
     return launched();
 }
 
+// ---- TrivialAugmentWide: one op per sample, then normalise (dmlb_image_trivial_augment) -----------------------------
+// (include/dmlb.h states the rule.)  One thread-block cluster per sample; CTA r of a cluster of n writes elements
+// [r S / n, (r + 1) S / n) of the sample's output in memory order (image_store_run).  Contrast, AutoContrast and
+// Equalize first reduce their statistics over pixels [r P / n, (r + 1) P / n) into the CTA's shared memory (a 128-bit
+// integer sum, per-channel min / max, per-channel 256-bin histograms), then every CTA folds the cluster's partials in
+// rank order through distributed shared memory between two cluster.sync(): exact integer and min / max folds, so the
+// result does not depend on the launch geometry.  Every CTA of a cluster holds the same sample, so the branch into
+// that phase is uniform.  Geometric ops and Sharpness gather from the sample, which sits in L2 at these sizes.
+
+namespace cg = cooperative_groups;
+
+constexpr int kTaThreads = 256;
+constexpr int kTaWarps = kTaThreads / 32;
+constexpr int kTaMaxCluster = 8;              // the portable cluster size
+constexpr int kTaPixelsPerCta = 4096;         // cluster size = ceil(h w / this), at most kTaMaxCluster
+constexpr int kTaMaxSide = 32768;             // h, w
+constexpr long long kTaMaxPixels = 1LL << 24; // h w: C h w fits an int run, the contrast sum fits 120 bits
+constexpr long long kTaMaxBatch = (1LL << 31) / kTaMaxCluster - 1;  // the grid is batch * cluster CTAs
+enum { kTaIdentity, kTaShearX, kTaShearY, kTaTranslateX, kTaTranslateY, kTaRotate, kTaBrightness, kTaColor,
+       kTaContrast, kTaSharpness, kTaPosterize, kTaSolarize, kTaAutoContrast, kTaEqualize, kTaOps };
+
+struct TaArgs {
+    const float *src;
+    const int *ops;
+    void *out;
+    long long S;  // C h w
+    int C, h, w, nhwc, bilinear;
+    float mean[4], std[4];
+};
+
+struct TaShared {
+    unsigned int hist[3][256];  // this CTA's histograms (read by the cluster)
+    unsigned int total[3][256]; // the cluster's
+    float lut[3][256];          // Equalize: fp32 output of every uint8 level
+    __int128 wsum[kTaWarps];
+    float wmin[kTaWarps][3], wmax[kTaWarps][3];
+    __int128 sum;               // this CTA's contrast sum
+    float mn[3], mx[3];         // this CTA's min / max
+    float cmin[3], cinv[3];     // AutoContrast: the subtrahend and divisor of every channel
+    float mean;                 // Contrast: the mean gray
+};
+static_assert(sizeof(TaShared) <= 227 * 1024, "the TrivialAugment CTA must fit the opt-in shared memory of sm_90");
+
+// trunc(f) as a 128-bit integer, exact for |f| < 2^127.
+__device__ __forceinline__ __int128 f32_trunc_i128(float f) {
+    if (fabsf(f) < 9.223372036854775808e18f) return (__int128)__float2ll_rz(f);
+    const uint32_t b = __float_as_uint(f);
+    const __int128 m = (__int128)((b & 0x7fffffu) | 0x800000u) << ((int)((b >> 23) & 0xffu) - 150);
+    return (b >> 31) ? -m : m;
+}
+
+// The fp64 RNE rounding of v.
+__device__ __forceinline__ double i128_to_f64(__int128 v) {
+    const bool neg = v < 0;
+    const unsigned __int128 u = neg ? (unsigned __int128)0 - (unsigned __int128)v : (unsigned __int128)v;
+    const unsigned long long hi = (unsigned long long)(u >> 64);
+    if (hi == 0) return neg ? -__ull2double_rn((unsigned long long)u) : __ull2double_rn((unsigned long long)u);
+    const int n = 64 - __clzll((long long)hi);  // u has 64 + n bits: keep the top 64, the rest as a sticky bit
+    const unsigned long long top = (unsigned long long)(u >> n) | (unsigned long long)((u << (128 - n)) != 0);
+    const double d = ldexp(__ull2double_rn(top), n);
+    return neg ? -d : d;
+}
+
+__device__ __forceinline__ float ta_clamp01(float v) { return v < 0.0f ? 0.0f : (v > 1.0f ? 1.0f : v); }
+
+// to_dtype(uint8) of torchvision: trunc(v * fl32(255.999)), clamped to [0, 255] (NaN -> 0)
+__device__ __forceinline__ int ta_quantize(float v) {
+    const float t = __fmul_rn(v, (float)255.999);
+    return t >= 255.0f ? 255 : (t > 0.0f ? (int)t : 0);
+}
+
+// One sample: its op and the per-sample constants, value(e) of output element e.
+template <bool kBf16>
+struct TaSample {
+    const float *src;
+    const TaShared *s;
+    const float *mean, *std;
+    int op, C, h, w, P, nhwc, bilinear, nan, rot;  // rot: 0 none, else rot90 k = rot (4 = identity)
+    float mag, f_mul, f_alpha, r[6];
+
+    __device__ __forceinline__ float in(int c, int y, int x) const {
+        const int p = y * w + x;
+        return __ldg(src + (nhwc ? (long long)p * C + c : (long long)c * P + p));
+    }
+    __device__ __forceinline__ float tap(int c, int y, int x) const {
+        return (unsigned)y < (unsigned)h && (unsigned)x < (unsigned)w ? in(c, y, x) : 0.0f;
+    }
+    __device__ __forceinline__ float gray(int y, int x) const {  // ATen fuses the two add_(alpha=) into FMAs
+        if (C == 1) return in(0, y, x);
+        const float l = __fmul_rn(in(0, y, x), (float)0.2989);
+        return __fmaf_rn(in(2, y, x), (float)0.114, __fmaf_rn(in(1, y, x), (float)0.587, l));
+    }
+    __device__ float geometric(int c, int y, int x) const {
+        if (rot) {
+            if (rot == 1) return in(c, x, w - 1 - y);
+            if (rot == 2) return in(c, h - 1 - y, w - 1 - x);
+            if (rot == 3) return in(c, h - 1 - x, y);
+            return in(c, y, x);
+        }
+        const float bx = (float)x - 0.5f * (float)(w - 1), by = (float)y - 0.5f * (float)(h - 1);
+        const float gx = __fadd_rn(__fmaf_rn(by, r[1], __fmul_rn(bx, r[0])), r[2]);
+        const float gy = __fadd_rn(__fmaf_rn(by, r[4], __fmul_rn(bx, r[3])), r[5]);
+        const float ix = __fsub_rn(__fmul_rn(__fadd_rn(gx, 1.0f), 0.5f * (float)w), 0.5f);
+        const float iy = __fsub_rn(__fmul_rn(__fadd_rn(gy, 1.0f), 0.5f * (float)h), 0.5f);
+        if (!bilinear) {
+            const float fx = rintf(ix), fy = rintf(iy);
+            return fx >= 0.0f && fx < (float)w && fy >= 0.0f && fy < (float)h ? in(c, (int)fy, (int)fx) : 0.0f;
+        }
+        const float x0 = floorf(ix), y0 = floorf(iy);
+        if (!(x0 >= -1.0f && x0 < (float)w && y0 >= -1.0f && y0 < (float)h)) return 0.0f;  // every tap outside
+        const float dx = __fsub_rn(ix, x0), dy = __fsub_rn(iy, y0);
+        const float ex = __fsub_rn(1.0f, dx), sy = __fsub_rn(1.0f, dy);
+        const int xi = (int)x0, yi = (int)y0;
+        float v = __fmul_rn(tap(c, yi, xi), __fmul_rn(sy, ex));
+        v = __fadd_rn(v, __fmul_rn(tap(c, yi, xi + 1), __fmul_rn(sy, dx)));
+        v = __fadd_rn(v, __fmul_rn(tap(c, yi + 1, xi), __fmul_rn(dy, ex)));
+        return __fadd_rn(v, __fmul_rn(tap(c, yi + 1, xi + 1), __fmul_rn(dy, dx)));
+    }
+    __device__ float sharpen(int c, int y, int x) const {
+        const float v = in(c, y, x);
+        if (h <= 2 || w <= 2) return v;
+        if (y == 0 || x == 0 || y == h - 1 || x == w - 1) return ta_clamp01(v);
+        const float a = (float)(1.0 / 13.0), b = (float)(5.0 / 13.0);
+        float acc = __fmul_rn(in(c, y - 1, x - 1), a);
+#pragma unroll
+        for (int k = 1; k < 9; ++k) {
+            const int dy = k / 3 - 1, dx = k % 3 - 1;
+            acc = __fadd_rn(acc, __fmul_rn(in(c, y + dy, x + dx), k == 4 ? b : a));
+        }
+        return ta_clamp01(__fmaf_rn(__fsub_rn(acc, v), f_alpha, v));  // add_(alpha=): fused
+    }
+    __device__ float op_value(int c, int y, int x) const {
+        switch (op) {
+            case kTaIdentity: return in(c, y, x);
+            case kTaBrightness: return ta_clamp01(__fmul_rn(in(c, y, x), f_mul));
+            case kTaColor:
+                if (C == 1) return in(c, y, x);
+                return ta_clamp01(__fmaf_rn(gray(y, x), f_alpha, __fmul_rn(in(c, y, x), f_mul)));
+            case kTaContrast: return ta_clamp01(__fmaf_rn(s->mean, f_alpha, __fmul_rn(in(c, y, x), f_mul)));
+            case kTaSharpness: return sharpen(c, y, x);
+            case kTaPosterize: {
+                const float levels = (float)(1 << (int)mag);
+                const float q = floorf(__fmul_rn(in(c, y, x), levels));
+                return __fmul_rn(q < 0.0f ? 0.0f : (q > levels - 1.0f ? levels - 1.0f : q), 1.0f / levels);
+            }
+            case kTaSolarize: {
+                const float v = in(c, y, x);
+                return v >= mag ? __fsub_rn(1.0f, v) : v;
+            }
+            case kTaAutoContrast: return ta_clamp01(__fdiv_rn(__fsub_rn(in(c, y, x), s->cmin[c]), s->cinv[c]));
+            case kTaEqualize: return s->lut[c][ta_quantize(in(c, y, x))];
+            default: return geometric(c, y, x);
+        }
+    }
+    __device__ __forceinline__ uint32_t value(long long e) const {
+        int c, p;
+        if (nhwc) {
+            p = (int)(e / C), c = (int)(e - (long long)p * C);
+        } else {
+            c = (int)(e / P), p = (int)(e - (long long)c * P);
+        }
+        if (nan) return kBf16 ? 0x7fc0u : 0x7fc00000u;
+        const int y = p / w;
+        const float v = __fdiv_rn(__fsub_rn(op_value(c, y, p - y * w), mean[c]), std[c]);
+        return kBf16 ? (uint32_t)f32_to_bf16(v) : __float_as_uint(v);
+    }
+};
+
+template <bool kBf16>
+struct TaCursor {
+    const TaSample<kBf16> &s;
+    long long e;
+    __device__ __forceinline__ uint32_t next() { return s.value(e++); }
+};
+
+// The cluster's statistics of the sample's op (Contrast, AutoContrast, Equalize) into s; every CTA calls it.
+template <bool kBf16>
+__device__ void ta_statistics(const TaSample<kBf16> &t, TaShared &s, cg::cluster_group &cluster) {
+    const int rank = (int)cluster.block_rank(), n = (int)cluster.num_blocks();
+    const int p0 = (int)((long long)t.P * rank / n), p1 = (int)((long long)t.P * (rank + 1) / n);
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    if (t.op == kTaEqualize) {
+        for (int k = threadIdx.x; k < 3 * 256; k += blockDim.x) (&s.hist[0][0])[k] = 0;
+        __syncthreads();
+        for (int p = p0 + threadIdx.x; p < p1; p += blockDim.x)
+            for (int c = 0; c < t.C; ++c) atomicAdd(&s.hist[c][ta_quantize(t.in(c, p / t.w, p % t.w))], 1u);
+    } else if (t.op == kTaContrast) {
+        __int128 acc = 0;
+        for (int p = p0 + threadIdx.x; p < p1; p += blockDim.x) {
+            float g = t.gray(p / t.w, p % t.w);
+            g = g != g ? 0.0f : fminf(fmaxf(g, -2147483648.0f), 2147483648.0f);
+            acc += f32_trunc_i128(__fmul_rn(g, 18446744073709551616.0f));
+        }
+        for (int o = 16; o; o >>= 1) {
+            const unsigned long long lo = __shfl_down_sync(0xffffffffu, (unsigned long long)acc, o);
+            const unsigned long long hi = __shfl_down_sync(0xffffffffu, (unsigned long long)((unsigned __int128)acc >> 64), o);
+            acc += (__int128)(((unsigned __int128)hi << 64) | lo);
+        }
+        if (lane == 0) s.wsum[warp] = acc;
+        __syncthreads();
+        if (threadIdx.x == 0) {
+            __int128 sum = 0;
+            for (int k = 0; k < kTaWarps; ++k) sum += s.wsum[k];
+            s.sum = sum;
+        }
+    } else {  // AutoContrast: NaN values are not counted (fminf / fmaxf)
+        float mn[3] = {INFINITY, INFINITY, INFINITY}, mx[3] = {-INFINITY, -INFINITY, -INFINITY};
+        for (int p = p0 + threadIdx.x; p < p1; p += blockDim.x)
+            for (int c = 0; c < t.C; ++c) {
+                const float v = t.in(c, p / t.w, p % t.w);
+                mn[c] = fminf(mn[c], v), mx[c] = fmaxf(mx[c], v);
+            }
+        for (int c = 0; c < 3; ++c) {
+            for (int o = 16; o; o >>= 1) {
+                mn[c] = fminf(mn[c], __shfl_down_sync(0xffffffffu, mn[c], o));
+                mx[c] = fmaxf(mx[c], __shfl_down_sync(0xffffffffu, mx[c], o));
+            }
+            if (lane == 0) s.wmin[warp][c] = mn[c], s.wmax[warp][c] = mx[c];
+        }
+        __syncthreads();
+        if (threadIdx.x < 3) {
+            float a = INFINITY, b = -INFINITY;
+            for (int k = 0; k < kTaWarps; ++k) a = fminf(a, s.wmin[k][threadIdx.x]), b = fmaxf(b, s.wmax[k][threadIdx.x]);
+            s.mn[threadIdx.x] = a, s.mx[threadIdx.x] = b;
+        }
+    }
+    cluster.sync();  // every CTA's partials are complete
+    if (t.op == kTaEqualize) {
+        for (int k = threadIdx.x; k < t.C * 256; k += blockDim.x) {
+            unsigned int v = 0;
+            for (int r = 0; r < n; ++r) v += (&cluster.map_shared_rank(&s, r)->hist[0][0])[k];
+            (&s.total[0][0])[k] = v;
+        }
+    } else if (t.op == kTaContrast) {
+        if (threadIdx.x == 0) {
+            __int128 sum = 0;
+            for (int r = 0; r < n; ++r) sum += cluster.map_shared_rank(&s, r)->sum;
+            s.mean = (float)(i128_to_f64(sum) * 0x1p-64 / (double)t.P);
+        }
+    } else if (threadIdx.x < t.C) {
+        const int c = threadIdx.x;
+        float a = INFINITY, b = -INFINITY;
+        for (int r = 0; r < n; ++r) {
+            const TaShared *q = cluster.map_shared_rank(&s, r);
+            a = fminf(a, q->mn[c]), b = fmaxf(b, q->mx[c]);
+        }
+        s.cmin[c] = a == b ? 0.0f : a;
+        s.cinv[c] = a == b ? 1.0f : __fsub_rn(b, a);
+    }
+    cluster.sync();  // no CTA leaves while another reads its shared memory
+    if (t.op == kTaEqualize && threadIdx.x < t.C) {  // torchvision's lut, one channel per thread
+        const int c = threadIdx.x;
+        unsigned int cum = 0, last = 0;
+        for (int k = 0; k < 256; ++k)
+            if (s.total[c][k]) last = k;
+        const unsigned int step = ((unsigned int)t.P - s.total[c][last]) / 255u;
+        for (int k = 0; k < 256; ++k) {
+            unsigned int level = (unsigned int)k;
+            if (step) {
+                level = k == 0 ? 0u : min((cum + step / 2) / step, 255u);
+                cum += s.total[c][k];
+            }
+            s.lut[c][k] = __fmul_rn((float)level, (float)(1.0 / 255.0));
+        }
+    }
+    __syncthreads();
+}
+
+template <bool kBf16>
+__global__ void __launch_bounds__(kTaThreads) image_trivial_augment_kernel(const TaArgs a) {
+    __shared__ TaShared s;
+    cg::cluster_group cluster = cg::this_cluster();
+    const int n = (int)cluster.num_blocks(), rank = (int)cluster.block_rank();
+    const long long i = blockIdx.x / n;
+    const int *row = a.ops + 8 * i;
+    TaSample<kBf16> t;
+    t.src = a.src + i * a.S;
+    t.s = &s;
+    t.mean = a.mean, t.std = a.std;
+    t.C = a.C, t.h = a.h, t.w = a.w, t.P = a.h * a.w, t.nhwc = a.nhwc, t.bilinear = a.bilinear;
+    t.op = __ldg(row);
+    t.mag = __int_as_float(__ldg(row + 1));
+    for (int k = 0; k < 6; ++k) t.r[k] = __fdiv_rn(__int_as_float(__ldg(row + 2 + k)), 0.5f * (float)(k < 3 ? a.w : a.h));
+    const double factor = 1.0 + (double)t.mag;
+    t.f_mul = (float)factor, t.f_alpha = (float)(1.0 - factor);
+    t.rot = 0;
+    if (t.op == kTaRotate) {  // torchvision rotate's exact paths, on python's angle % 360
+        double deg = fmod((double)t.mag, 360.0);
+        if (deg < 0.0) deg += 360.0;
+        t.rot = deg == 0.0 ? 4 : deg == 180.0 ? 2 : a.h != a.w ? 0 : deg == 90.0 ? 1 : deg == 270.0 ? 3 : 0;
+    }
+    t.nan = t.op < 0 || t.op >= kTaOps || __ldg(t.src) != __ldg(t.src) ||
+            (t.op == kTaPosterize && !(t.mag > -1.0f && t.mag < 9.0f));
+    if (!t.nan && (t.op == kTaContrast || t.op == kTaAutoContrast || t.op == kTaEqualize)) ta_statistics(t, s, cluster);
+    const long long e0 = a.S * rank / n, e1 = a.S * (rank + 1) / n;
+    image_store_run<kBf16>(a.out, i * a.S + e0, (int)(e1 - e0), [&](int k) { return TaCursor<kBf16>{t, e0 + k}; });
+}
+
+static int ta_cluster(long long pixels) {
+    const long long n = (pixels + kTaPixelsPerCta - 1) / kTaPixelsPerCta;
+    return (int)(n < kTaMaxCluster ? n : kTaMaxCluster);
+}
+
+template <bool kBf16>
+static int launch_trivial_augment(long long batch, int cluster, cudaStream_t st, const TaArgs &a) {
+    cudaLaunchConfig_t cfg = {};
+    cfg.gridDim = dim3((unsigned)(batch * cluster));
+    cfg.blockDim = dim3(kTaThreads);
+    cfg.stream = st;
+    cudaLaunchAttribute attr;
+    attr.id = cudaLaunchAttributeClusterDimension;
+    attr.val.clusterDim.x = (unsigned)cluster, attr.val.clusterDim.y = 1, attr.val.clusterDim.z = 1;
+    cfg.attrs = &attr;
+    cfg.numAttrs = 1;
+    const cudaError_t e = cudaLaunchKernelEx(&cfg, image_trivial_augment_kernel<kBf16>, a);
+    const int r = launched();
+    return e != cudaSuccess ? -(int)e : r;
+}
+
 }  // namespace dmlb
 
 using namespace dmlb;
@@ -839,6 +1160,33 @@ int dmlb_image_mix(const float *src, const int64_t *idx, const int64_t *labels, 
     cudaStream_t st = (cudaStream_t)stream;
     if (out_bf16) return vec ? launch_mix<true, 8>(grid, st, a) : launch_mix<true, 1>(grid, st, a);
     return vec ? launch_mix<false, 4>(grid, st, a) : launch_mix<false, 1>(grid, st, a);
+}
+
+int dmlb_image_trivial_augment(const float *src, const int32_t *ops, int64_t batch, int32_t C, int32_t h, int32_t w,
+                               int bilinear, const dmlb_image_norm *norm, void *out, int out_bf16, int channels_last,
+                               void *stream) {
+    if (batch < 0 || batch > kTaMaxBatch || !norm || (C != 1 && C != 3) || h < 1 || w < 1 || h > kTaMaxSide ||
+        w > kTaMaxSide || (long long)h * w > kTaMaxPixels || (bilinear != 0 && bilinear != 1))
+        return DMLB_EINVAL;
+    TaArgs a;
+    if (!pack_norm(norm, C, a.mean, a.std)) return DMLB_EINVAL;
+    if (batch > 0 && (!src || !ops || !out)) return DMLB_EINVAL;
+    const long long S = (long long)C * h * w;
+    const uintptr_t s0 = (uintptr_t)src, s1 = s0 + (uintptr_t)(batch * S * 4);
+    const uintptr_t o0 = (uintptr_t)out, o1 = o0 + (uintptr_t)(batch * S * (out_bf16 ? 2 : 4));
+    if (batch > 0 && s0 < o1 && o0 < s1) return DMLB_EINVAL;
+    if ((s0 & 3) != 0 || ((uintptr_t)ops & 3) != 0 || (o0 & (out_bf16 ? 1 : 3)) != 0) return DMLB_EALIGN;
+    if (batch == 0) return DMLB_OK;
+
+    a.src = src;
+    a.ops = ops;
+    a.out = out;
+    a.S = S;
+    a.C = C, a.h = h, a.w = w, a.nhwc = channels_last ? 1 : 0, a.bilinear = bilinear;
+    const int cluster = ta_cluster((long long)h * w);
+    cudaStream_t st = (cudaStream_t)stream;
+    return out_bf16 ? launch_trivial_augment<true>(batch, cluster, st, a)
+                    : launch_trivial_augment<false>(batch, cluster, st, a);
 }
 
 }  // extern "C"

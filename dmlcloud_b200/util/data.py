@@ -30,6 +30,8 @@ or device tables (one per epoch).  They all come from one counter hash:
                the offsets from 4 + 3a
       32..62   erase_boxes: erased when u53(word 32) < p; attempt a takes the area from word 33 + 3a, the log aspect
                ratio from 34 + 3a, the offsets from 35 + 3a
+      63       ta_ops: TrivialAugmentWide's op = below(word 63 >> 32, 14) and bin = below(word 63 & 0xffffffff, bins)
+      64       ta_ops: a signed op's magnitude is negated when u53(word 64) <= 0.5
   batch hash hb = mix(mix(e ^ (rank + g + 2^63)) ^ (batch + g)), e = mix(mix(seed + g) ^ (epoch + g)) (batch_hash); a
              row's hash is mix(e ^ (row + g)) with row < 2^63 and mix is a bijection, so hb is never a row's hash.
              mix_batch_params takes the MixUp / CutMix choice from mix(hb + g) >> 63, CutMix's centre from
@@ -305,11 +307,13 @@ def _image_hwc(images):
 class _DeviceImageBatches(DeviceShardedDataset):
     """What the colour-image datasets share: normalisation, layout, batch mixing and the batch loop.  A subclass checks
     its geometry, passes its output size `crop` and supplies epoch_table() (numpy int32, one row per sample of this
-    rank's epoch, in iteration order) and _launch(view, table_rows, x), which writes the images of `view` into x."""
+    rank's epoch, in iteration order) and _launch(view, table_rows, x, norm), which writes the images of `view` into x
+    normalised by the ImageNorm `norm`."""
 
     def __init__(self, images, labels, batch_size, mean, std, crop, hflip, memory_format, out_dtype, shuffle,
                  even_shards, seed, aug_seed, rank, world_size, device, drop_last, mixup_alpha, cutmix_alpha,
-                 num_classes, random_erase, erase_scale, erase_ratio, erase_value):
+                 num_classes, random_erase, erase_scale, erase_ratio, erase_value, trivial_augment, ta_bins,
+                 ta_interpolation):
         if memory_format not in (torch.contiguous_format, torch.channels_last):
             raise ValueError('memory_format must be torch.contiguous_format or torch.channels_last')
         super().__init__(images, labels, batch_size, shuffle=shuffle, even_shards=even_shards, seed=seed, rank=rank,
@@ -353,6 +357,21 @@ class _DeviceImageBatches(DeviceShardedDataset):
         self._mixing = mixing or self.random_erase > 0.0
         if self._mixing and max(self.crop) > 32768:
             raise ValueError(f'crop {self.crop}: dmlb_image_mix takes sides of at most 32768')
+        self.trivial_augment = bool(trivial_augment)
+        self.ta_bins, self.ta_interpolation = int(ta_bins), ta_interpolation
+        if self.trivial_augment:
+            if C not in (1, 3):
+                raise ValueError(f'TrivialAugmentWide takes 1 or 3 channels, got {C}')
+            if self.ta_bins < 2:
+                raise ValueError(f'ta_bins must be >= 2, got {ta_bins}')
+            if ta_interpolation not in ('nearest', 'bilinear'):
+                raise ValueError(f"ta_interpolation must be 'nearest' or 'bilinear', got {ta_interpolation!r}")
+            h, w = self.crop
+            if max(h, w) > 32768 or h * w > 1 << 24:
+                raise ValueError(f'crop {self.crop}: TrivialAugmentWide takes sides of at most 32768 and at most '
+                                 '2^24 pixels')
+            self._ta_magnitudes = ta_magnitudes(self.ta_bins)
+            self._identity = self._N.ImageNorm.of([0.0] * C, [1.0] * C)
 
     def _shard_rows(self):
         """This rank's dataset rows for the current epoch in iteration order (numpy)."""
@@ -366,6 +385,22 @@ class _DeviceImageBatches(DeviceShardedDataset):
             return np.zeros((len(rows), 5), dtype=np.int32)
         return erase_boxes(rows, self.crop[0], self.crop[1], self.random_erase, self.erase_scale, self.erase_ratio,
                            self.aug_seed, self.epoch)
+
+    def epoch_ta_ops(self):
+        """int32 [shard_len(), 8] numpy {op, magnitude, theta0..5} (ta_ops) of this rank's samples this epoch, in
+        iteration order, the floats by their fp32 bit patterns."""
+        return ta_ops(self._shard_rows(), self.ta_bins, self.crop[0], self.crop[1], self.aug_seed, self.epoch,
+                      self._ta_magnitudes)
+
+    def _augment(self, ops, scratch, x):
+        """TrivialAugmentWide and the normalisation of the identity-normalised fp32 `scratch` into x (one launch)."""
+        N = self._N
+        _, _, C = self.item_shape
+        h, w = self.crop
+        N.check(N.cuda_lib(self.device.index).dmlb_image_trivial_augment(
+            scratch.data_ptr(), ops.data_ptr(), ops.shape[0], C, h, w, int(self.ta_interpolation == 'bilinear'),
+            self._norm, x.data_ptr(), int(x.dtype == torch.bfloat16), int(self.memory_format == torch.channels_last),
+            N.stream_ptr()), 'image_trivial_augment')
 
     def batch_params(self, batch):
         """{'mode', 'lam', 'lam_adjusted', 'box'} of this rank's batch number `batch` this epoch (mix_batch_params)."""
@@ -411,17 +446,29 @@ class _DeviceImageBatches(DeviceShardedDataset):
             N.stream_ptr()), 'image_mix')
         return x, y
 
+    def _images(self, view, rows, ops, x):
+        """The images of `view` into x: _launch alone, or (TrivialAugmentWide) _launch into an fp32 scratch batch with
+        the identity normalisation, which dmlb_image_trivial_augment augments and normalises into x."""
+        if ops is None:
+            self._launch(view, rows, x, self._norm)
+            return
+        scratch = self._empty(view.numel(), torch.float32)
+        self._launch(view, rows, scratch, self._identity)
+        self._augment(ops, scratch, x)
+
     def __iter__(self):
-        """The epoch's batches: _launch writes the images of each batch into x, then the labels are gathered, or (batch
-        mixing) x is an fp32 scratch batch that dmlb_image_mix erases and mixes into the yielded batch together with
-        its targets."""
+        """The epoch's batches: _images writes the images of each batch into x, then the labels are gathered, or
+        (batch mixing) x is an fp32 scratch batch that dmlb_image_mix erases and mixes into the yielded batch together
+        with its targets."""
         N = self._N
         lib = N.cuda_lib(self.device.index)
         idx, table = self.augment_params()
         count = idx.numel()
-        erase = None
+        erase = ops = None
         if self.random_erase > 0.0:
             erase = torch.from_numpy(self.epoch_erase_boxes()).to(self.device)
+        if self.trivial_augment:
+            ops = torch.from_numpy(self.epoch_ta_ops()).to(self.device)
         for start in range(0, count, self.batch_size):
             b = min(self.batch_size, count - start)
             if b < self.batch_size and self.drop_last:
@@ -429,13 +476,13 @@ class _DeviceImageBatches(DeviceShardedDataset):
             view, rows = idx[start:start + b], table[start:start + b]
             if self._mixing:
                 scratch = self._empty(b, torch.float32)
-                self._launch(view, rows, scratch)
+                self._images(view, rows, None if ops is None else ops[start:start + b], scratch)
                 yield self._mixed(view, scratch, None if erase is None else erase[start:start + b],
                                   start // self.batch_size)
                 continue
             x = self._empty(b)
             y = torch.empty(b, dtype=torch.int64, device=self.device)
-            self._launch(view, rows, x)
+            self._images(view, rows, None if ops is None else ops[start:start + b], x)
             N.check(lib.dmlb_shard_gather_i64(self.labels.data_ptr(), view.data_ptr(), b, y.data_ptr(), N.stream_ptr()),
                     'shard_gather_i64')
             yield x, y
@@ -466,13 +513,21 @@ class DeviceImageDataset(_DeviceImageBatches):
     loss, as in torchvision); with erasing alone they are (x, int64 y).  Either way each batch is two launches: the image
     kernel writes an fp32 scratch batch and dmlb_image_mix erases, mixes and writes x and the targets.
     mix_params() gives the erase table and the per-batch draws of the epoch.
+
+    TrivialAugmentWide (torchvision's `--auto-augment ta_wide`, off by default):
+      trivial_augment  TrivialAugmentWide(num_magnitude_bins=ta_bins, interpolation=ta_interpolation, fill=None) of
+                    torchvision v2 on every sample's float image in [0, 1], after the crop and flip and before
+                    Normalize (and before the batch mixing); ta_interpolation is 'nearest' or 'bilinear'; C must be
+                    1 or 3.  A sample's op and magnitude depend only on (aug_seed, epoch, dataset index) (ta_ops);
+                    epoch_ta_ops() gives the epoch's table.  It adds one launch per batch: the image kernel writes an
+                    fp32 scratch batch with mean 0 and std 1, which dmlb_image_trivial_augment augments and normalises.
     """
 
     def __init__(self, images, labels, batch_size, mean, std, crop=None, padding=0, random_crop=True, hflip=False,
                  memory_format=torch.contiguous_format, out_dtype=torch.float32, shuffle=True, even_shards=True, seed=0,
                  aug_seed=None, rank=None, world_size=None, device=None, drop_last=False, mixup_alpha=0.0,
                  cutmix_alpha=0.0, num_classes=None, random_erase=0.0, erase_scale=(0.02, 0.33), erase_ratio=(0.3, 3.3),
-                 erase_value=0.0):
+                 erase_value=0.0, trivial_augment=False, ta_bins=31, ta_interpolation='nearest'):
         H, W, _ = _image_hwc(images)
         self.padding = int(padding)
         if crop is None:
@@ -483,7 +538,8 @@ class DeviceImageDataset(_DeviceImageBatches):
         self.random_crop = bool(random_crop)
         super().__init__(images, labels, batch_size, mean, std, crop, hflip, memory_format, out_dtype, shuffle,
                          even_shards, seed, aug_seed, rank, world_size, device, drop_last, mixup_alpha, cutmix_alpha,
-                         num_classes, random_erase, erase_scale, erase_ratio, erase_value)
+                         num_classes, random_erase, erase_scale, erase_ratio, erase_value, trivial_augment, ta_bins,
+                         ta_interpolation)
 
     def epoch_table(self):
         """int32 [shard_len(), 3] numpy {top, left, flipped} (crop_windows) of this rank's samples this epoch, in
@@ -492,12 +548,12 @@ class DeviceImageDataset(_DeviceImageBatches):
         return crop_windows(self._shard_rows(), H, W, *self.crop, self.padding, self.random_crop, self.hflip,
                             self.aug_seed, self.epoch)
 
-    def _launch(self, view, windows, x):
+    def _launch(self, view, windows, x, norm):
         N = self._N
         H, W, C = self.item_shape
         N.check(N.cuda_lib(self.device.index).dmlb_image_batch_u8(
             self.images.data_ptr(), view.data_ptr(), windows.data_ptr(), view.numel(), H, W, C, *self.crop,
-            self.padding, self._norm, x.data_ptr(), int(x.dtype == torch.bfloat16),
+            self.padding, norm, x.data_ptr(), int(x.dtype == torch.bfloat16),
             int(self.memory_format == torch.channels_last), N.stream_ptr()), 'image_batch_u8')
 
 
@@ -612,6 +668,78 @@ def erase_boxes(rows, h, w, p, scale, ratio, seed, epoch):
     return box.astype(np.int32)
 
 
+TA_WORD = 63  # the TrivialAugmentWide words of a row, 63 and 64, follow the erase words
+TA_OPS = ('Identity', 'ShearX', 'ShearY', 'TranslateX', 'TranslateY', 'Rotate', 'Brightness', 'Color', 'Contrast',
+          'Sharpness', 'Posterize', 'Solarize', 'AutoContrast', 'Equalize')  # torchvision's _AUGMENTATION_SPACE order
+_TA_SIGNED = (np.arange(14) >= 1) & (np.arange(14) <= 9)  # ShearX .. Sharpness take a random sign
+
+
+def ta_magnitudes(bins):
+    """fp32 [14, bins]: TrivialAugmentWide's magnitude of every op and bin, computed as torchvision computes its
+    tables (torch.linspace, and the Posterize formula); 0 for the ops without one."""
+    table = torch.zeros(14, bins)
+    for op, (a, b) in {1: (0.0, 0.99), 2: (0.0, 0.99), 3: (0.0, 32.0), 4: (0.0, 32.0), 5: (0.0, 135.0), 6: (0.0, 0.99),
+                       7: (0.0, 0.99), 8: (0.0, 0.99), 9: (0.0, 0.99), 11: (1.0, 0.0)}.items():
+        table[op] = torch.linspace(a, b, bins)
+    table[10] = (8 - (torch.arange(bins) / ((bins - 1) / 6))).round().int()
+    return table.numpy()
+
+
+def _inverse_affine(center, angle, translate, shear):
+    """torchvision's _get_inverse_affine_matrix at scale 1, restated in python fp64."""
+    rot, sx, sy = math.radians(angle), math.radians(shear[0]), math.radians(shear[1])
+    cx, cy = center
+    tx, ty = translate
+    a = math.cos(rot - sy) / math.cos(sy)
+    b = -(a * math.tan(sx) + math.sin(rot))
+    c = math.sin(rot - sy) / math.cos(sy)
+    d = math.cos(rot) - c * math.tan(sx)
+    m = [d, -b, 0.0, -c, a, 0.0]
+    m[2] += cx - m[0] * (cx + tx) - m[1] * (cy + ty)
+    m[5] += cy - m[3] * (cx + tx) - m[4] * (cy + ty)
+    return m
+
+
+def ta_theta(op, magnitude, h, w):
+    """fp32 [6]: the inverse affine matrix torchvision's affine (Shear about the corner, Translate by int(magnitude))
+    or rotate (about the centre, by -(magnitude % 360)) forms for geometric op `op` on an h x w sample, rounded to
+    fp32 as torch.tensor(matrix, dtype=float32) does; zeros for the other ops."""
+    if op in (1, 2):
+        deg = math.degrees(math.atan(magnitude))
+        m = _inverse_affine([-w * 0.5, -h * 0.5], 0.0, [0.0, 0.0], [deg, 0.0] if op == 1 else [0.0, deg])
+    elif op in (3, 4):
+        t = float(int(magnitude))
+        m = _inverse_affine([0.0, 0.0], 0.0, [t, 0.0] if op == 3 else [0.0, t], [0.0, 0.0])
+    elif op == 5:
+        m = _inverse_affine([0.0, 0.0], -(magnitude % 360), [0.0, 0.0], [0.0, 0.0])
+    else:
+        m = [0.0] * 6
+    return np.asarray(m, dtype=np.float64).astype(np.float32)
+
+
+def ta_ops(rows, bins, h, w, seed, epoch, magnitudes=None):
+    """int32 [len(rows), 8] {op, magnitude, theta0..5}, the floats by their fp32 bit patterns: TrivialAugmentWide's
+    draw for every row, op and bin from row word 63, the sign of a signed op's magnitude from word 64, theta the
+    ta_theta of the geometric ops on an h x w sample.  The draws are vectorised; the matrices are formed once per
+    distinct (op, magnitude)."""
+    mags = ta_magnitudes(bins) if magnitudes is None else magnitudes
+    hr = _row_hash(rows, seed, epoch)
+    w63 = _word(hr, TA_WORD)
+    op = _below(w63 >> np.uint64(32), 14)
+    mag = mags[op, _below(w63 & np.uint64(0xFFFFFFFF), bins)].astype(np.float32)
+    neg = _TA_SIGNED[op] & (_u53(hr, TA_WORD + 1) <= 0.5)
+    mag = np.where(neg, -mag, mag).astype(np.float32)
+    out = np.zeros((len(hr), 8), dtype=np.int32)
+    out[:, 0] = op
+    out[:, 1] = mag.view(np.int32)
+    geo = (op >= 1) & (op <= 5)
+    if geo.any():
+        keys, inverse = np.unique(np.stack([op[geo], mag[geo].view(np.int32)], axis=1), axis=0, return_inverse=True)
+        thetas = np.stack([ta_theta(int(o), float(np.int32(m).view(np.float32)), h, w) for o, m in keys])
+        out[geo, 2:] = thetas[inverse.reshape(-1)].view(np.int32)
+    return out
+
+
 _M64 = (1 << 64) - 1
 _G = int(_GAMMA)
 MIXUP, CUTMIX = 1, 2
@@ -714,14 +842,16 @@ class DeviceResizedImageDataset(_DeviceImageBatches):
     DeviceShardedDataset's.  The kernel takes image and resized sides of at most 32768, resizes at
     most 8x down on each axis and writes rows of at most 1024 values; the constructor refuses anything else.
     augment_params() gives the epoch's indices and boxes.  Batch mixing (random_erase, mixup_alpha, cutmix_alpha, ...)
-    is DeviceImageDataset's, on the size[0] x size[1] output.
+    and TrivialAugmentWide (trivial_augment, ta_bins, ta_interpolation) are DeviceImageDataset's, on the
+    size[0] x size[1] output.
     """
 
     def __init__(self, images, labels, batch_size, mean, std, size, scale=(0.08, 1.0), ratio=(3 / 4, 4 / 3),
                  random=True, resize=None, hflip=False, memory_format=torch.contiguous_format,
                  out_dtype=torch.float32, shuffle=True, even_shards=True, seed=0, aug_seed=None, rank=None,
                  world_size=None, device=None, drop_last=False, mixup_alpha=0.0, cutmix_alpha=0.0, num_classes=None,
-                 random_erase=0.0, erase_scale=(0.02, 0.33), erase_ratio=(0.3, 3.3), erase_value=0.0):
+                 random_erase=0.0, erase_scale=(0.02, 0.33), erase_ratio=(0.3, 3.3), erase_value=0.0,
+                 trivial_augment=False, ta_bins=31, ta_interpolation='nearest'):
         H, W, C = _image_hwc(images)
         size = (int(size), int(size)) if isinstance(size, (int, np.integer)) else tuple(int(v) for v in size)
         if len(size) != 2 or min(size) < 1:
@@ -753,7 +883,8 @@ class DeviceResizedImageDataset(_DeviceImageBatches):
             raise ValueError(f'size[1] * C = {size[1] * C} is above the 1024 values per output row the kernel takes')
         super().__init__(images, labels, batch_size, mean, std, size, hflip, memory_format, out_dtype, shuffle,
                          even_shards, seed, aug_seed, rank, world_size, device, drop_last, mixup_alpha, cutmix_alpha,
-                         num_classes, random_erase, erase_scale, erase_ratio, erase_value)
+                         num_classes, random_erase, erase_scale, erase_ratio, erase_value, trivial_augment, ta_bins,
+                         ta_interpolation)
 
     def epoch_table(self):
         """int32 [shard_len(), 5] numpy {top, left, height, width, flipped} of this rank's samples this epoch, in
@@ -766,10 +897,10 @@ class DeviceResizedImageDataset(_DeviceImageBatches):
         boxes[:, 4] = _flips(_row_hash(rows, self.aug_seed, self.epoch), self.hflip)
         return boxes
 
-    def _launch(self, view, boxes, x):
+    def _launch(self, view, boxes, x, norm):
         N = self._N
         H, W, C = self.item_shape
         N.check(N.cuda_lib(self.device.index).dmlb_image_resample_u8(
             self.images.data_ptr(), view.data_ptr(), boxes.data_ptr(), view.numel(), H, W, C, *self.resized,
-            *self.window, *self.crop, self._norm, x.data_ptr(), int(x.dtype == torch.bfloat16),
+            *self.window, *self.crop, norm, x.data_ptr(), int(x.dtype == torch.bfloat16),
             int(self.memory_format == torch.channels_last), N.stream_ptr()), 'image_resample_u8')

@@ -456,6 +456,53 @@ int dmlb_image_mix(const float *src, const int64_t *idx, const int64_t *labels, 
                    int32_t x1, int32_t x2, int32_t num_classes, void *out, int out_bf16, int channels_last,
                    void *targets, void *stream);
 
+/* TrivialAugmentWide: one op per sample on the float image in [0, 1], then per-channel normalise, one launch.
+ * torchvision v2's TrivialAugmentWide(fill=None) float kernels, with the operation order below (fl = one fp32
+ * rounding, fma = fused multiply-add where ATen's add_(alpha=) fuses it; every other operation is rounded once).
+ *   src : DEVICE fp32 logical [batch, C, h, w] (an image batch written with mean 0, std 1), NCHW (channels_last == 0)
+ *         or NHWC in memory; out has the same layout, fp32 or bf16 (RNE, rounded once at the end)
+ *   ops : DEVICE int32 [batch][8] {op, magnitude, theta0..theta5}, the floats by their fp32 bit patterns
+ *         (util/data.py ta_ops); bilinear: 0 nearest, 1 bilinear (the geometric ops)
+ * With m = magnitude, factor = 1 + m in fp64, mul = fl(factor), alpha = fl(1 - factor) (fp64, then rounded), v = the
+ * input value at (c, y, x), and clamp = clamp(., 0, 1) (NaN stays NaN), sample i's value is, by op:
+ *   0 Identity      v
+ *   1..4 ShearX, ShearY, TranslateX, TranslateY, and 5 Rotate (unless exact, below): grid_sample(zeros,
+ *                   align_corners=False) at theta, torchvision's inverse affine matrix: r = theta[0..2] / fl(w / 2),
+ *                   theta[3..5] / fl(h / 2); bx = x - (w - 1) / 2, by = y - (h - 1) / 2 (exact);
+ *                   gx = fl(fma(by, r1, fl(bx r0)) + r2), gy likewise with r3..r5 (ATen's bmm, bit for bit);
+ *                   ix = fl(fl(fl(gx + 1) * w / 2) - 0.5), iy likewise; nearest: the pixel at rint(ix, iy) (halves to
+ *                   even), 0 outside; bilinear: x0 = floor(ix), dx = fl(ix - x0), ex = fl(1 - dx) (dy, sy likewise),
+ *                   out = v00 fl(sy ex) + v01 fl(sy dx) + v10 fl(dy ex) + v11 fl(dy dx) in that order, 0 outside
+ *   5 Rotate exact: with a = m % 360 as python's fp64 modulo: a == 0 is Identity, a == 180 rot90(k=2), and on square
+ *                   samples a == 90 rot90(k=1), a == 270 rot90(k=3)
+ *   6 Brightness    clamp(fl(v mul))
+ *   7 Color         C = 1: v; C = 3: clamp(fma(gray, alpha, fl(v mul))), gray = fma(b, fl(.114), fma(g, fl(.587),
+ *                   fl(r fl(.2989))))  (torchvision's grayscale: mul then two add_(alpha=), fused)
+ *   8 Contrast      clamp(fma(mean, alpha, fl(v mul))), mean = fl(fl64(sum trunc(g 2^64)) 2^-64 / (h w)) with the sum
+ *                   exact in 128 bits over g = gray (C = 3) or v (C = 1) clamped to [-2^31, 2^31] (NaN counts 0)
+ *   9 Sharpness     h <= 2 or w <= 2: v; border pixels: clamp(v); inside: blur = the 3x3 taps in row-major order, each
+ *                   fl(v' fl(1/13)) (centre fl(5/13)) added with one rounding each; clamp(fma(fl(blur - v), alpha, v))
+ *  10 Posterize     bits = trunc(m) (0..8, else the sample is NaN), L = 2^bits: fl(clamp(floor(fl(v L)), 0, L - 1) / L)
+ *  11 Solarize      v >= m ? fl(1 - v) : v
+ *  12 AutoContrast  per channel min and max over the sample (NaN not counted); min == max: v (then clamp), else
+ *                   clamp(fl(fl(v - min) / fl(max - min)))
+ *  13 Equalize      per channel q = trunc(fl(v fl(255.999))) clamped to [0, 255] (NaN -> 0), torchvision's lut of the
+ *                   256-bin histogram of q (step = (h w - count of the last occupied bin) / 255; step == 0 keeps q),
+ *                   out = fl(lut[q] fl(1 / 255))
+ * then out = fl(fl(value - mean[c]) / std[c]).  Min, max, the histograms and the contrast sum are exact whatever the
+ * launch geometry.  Device data is not checked by the host; the kernel defines what it does with it: a sample whose
+ * first element is NaN, or whose op is outside 0..13, is written all quiet NaN.
+ * Launch: one thread-block cluster of ceil(h w / 4096) CTAs (at most 8) per sample; the statistics of ops 8, 12 and
+ * 13 are folded across the cluster through distributed shared memory (no atomics in global memory, no second launch).
+ * Accepted range (anything else: DMLB_EINVAL, nothing launched): C in {1, 3}; h, w in 1..32768 and h w <= 2^24;
+ * batch <= 2^28 - 1; bilinear in {0, 1}; std[c] != 0 for c < C; non-NULL norm, and src, ops, out when batch > 0;
+ * src and out not overlapping.  DMLB_EALIGN: src or ops not aligned to 4 bytes, out not to its element.  Every
+ * accepted argument set launches.  Out is written once with 16-byte stores between scalar heads and tails.
+ * Algorithmic bytes/sample: C h w * 4 read + C h w * (4 | 2) written + 32 B of op row. */
+int dmlb_image_trivial_augment(const float *src, const int32_t *ops, int64_t batch, int32_t C, int32_t h, int32_t w,
+                               int bilinear, const dmlb_image_norm *norm, void *out, int out_bf16, int channels_last,
+                               void *stream);
+
 #ifdef __cplusplus
 }
 #endif
