@@ -1,8 +1,10 @@
-"""Builds libdmlb.so in-tree with nvcc for sm_90a (H100; no torch headers: ~10 s, cross-compiles without a GPU).
+"""Builds libdmlb.so and libdmlb_layers.so in-tree with nvcc for sm_90a (H100; no torch headers: ~10 s, cross-compiles
+without a GPU).
 
     python -m dmlcloud_b200.csrc.build [--force] [--ptxas-v]
 
-The .so and its stamp are build products (git-ignored): a fresh checkout builds them once.
+The two libraries share one stamp: a change to either one's sources rebuilds both.  The .so files and the stamp are
+build products (git-ignored): a fresh checkout builds them once.
 """
 import hashlib
 import os
@@ -15,6 +17,9 @@ SOURCES = ['core.cu', 'bucket_kernels.cu', 'bucket_tma.cu', 'peer_comm.cu', 'met
            'optim_kernels.cu', 'vmm.cu']
 HEADERS = ['dmlb_common.cuh', 'peer_comm.cuh', 'metric_dev.cuh', '../../include/dmlb.h']
 LIB = HERE / 'libdmlb.so'
+LAYERS_SOURCES = ['layer_kernels.cu']  # model layers (include/dmlb_layers.h): a library of their own, own launch counter
+LAYERS_HEADERS = ['../../include/dmlb_layers.h']
+LAYERS_LIB = HERE / 'libdmlb_layers.so'
 STAMP = HERE / '.libdmlb.stamp'
 
 NVCC_FLAGS = [
@@ -34,7 +39,7 @@ def nvcc():
 
 def _digest():
     h = hashlib.sha256()
-    for name in SOURCES + HEADERS:
+    for name in SOURCES + HEADERS + LAYERS_SOURCES + LAYERS_HEADERS:
         h.update((HERE / name).read_bytes())
     h.update(' '.join(NVCC_FLAGS).encode())
     return h.hexdigest()
@@ -42,21 +47,22 @@ def _digest():
 
 def build(force=False, verbose=False, ptxas_v=False):
     digest = _digest()
-    if not force and LIB.exists() and STAMP.exists() and STAMP.read_text() == digest:
+    if not force and LIB.exists() and LAYERS_LIB.exists() and STAMP.exists() and STAMP.read_text() == digest:
         return LIB
-    cmd = [nvcc()] + NVCC_FLAGS + (['-Xptxas', '-v'] if ptxas_v else []) + \
-          ['-o', str(LIB)] + [str(HERE / s) for s in SOURCES]
-    if verbose:
-        print(' '.join(cmd), flush=True)
-    proc = subprocess.run(cmd, stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True)
-    if proc.returncode != 0:
-        raise RuntimeError('nvcc failed:\n' + proc.stdout)
-    if verbose or ptxas_v:
-        print(proc.stdout)
+    for lib, sources in ((LIB, SOURCES), (LAYERS_LIB, LAYERS_SOURCES)):
+        cmd = [nvcc()] + NVCC_FLAGS + (['-Xptxas', '-v'] if ptxas_v else []) + \
+              ['-o', str(lib)] + [str(HERE / s) for s in sources]
+        if verbose:
+            print(' '.join(cmd), flush=True)
+        proc = subprocess.run(cmd, stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True)
+        if proc.returncode != 0:
+            raise RuntimeError('nvcc failed:\n' + proc.stdout)
+        if verbose or ptxas_v:
+            print(proc.stdout)
     STAMP.write_text(digest)
     return LIB
 
 
 if __name__ == '__main__':
     build(force='--force' in sys.argv, verbose=True, ptxas_v='--ptxas-v' in sys.argv)
-    print(LIB)
+    print(LIB, LAYERS_LIB)

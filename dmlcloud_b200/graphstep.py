@@ -39,6 +39,11 @@ layout.  The communicator's sequence number and the exchange counter live in dev
 paths.  So rank 0 may replay the graph of its 8-sample last batch while rank 1 runs its 5-sample last batch as a flat
 step: both issue the same collective.  A step kind that issued a second collective, or none, would break this.
 
+Models of the small Conv3x3/ReLU/MaxPool -> Linear family (`layers.plan_of`) run as one forward and one backward kernel
+of libdmlb_layers.so inside `_one_step` (`TrainValStage.fused_layers`, on by default): the backward adds their gradients
+straight into the flat bucket.  Those launches are counted apart from libdmlb's (`layer_kernels_in_graph`), so
+`kernels_in_graph` stays the path's exchange and optimizer launches.
+
 Requirements: FlatAdam / FlatSGD, or torch optimizers constructed with `capturable=True` and no scheduler; `step()` must
 not synchronise with the host (no .item(), no printing of tensors) and must depend on the batch only through its
 signature (shapes, dtypes, python values), as any captured code must.
@@ -54,6 +59,7 @@ import torch.distributed as dist
 from torch.nn.parallel import DistributedDataParallel
 from torch.utils._pytree import tree_flatten, tree_unflatten
 
+from . import _layers as L
 from . import _native as N
 from .gradsync import WIRES, PeerComm, wire_bytes
 from .metrics import HostFeed, StepRing, _RingResult
@@ -113,6 +119,8 @@ class _ShapeGraph:
         self.leaves = None        # static inputs: device tensors (non-tensor leaves as the loader gave them)
         self.batch = None         # the same leaves in the loader's structure: what the step receives
         self.kernels = 0          # libdmlb kernels one replay re-runs
+        self.layer_kernels = 0    # libdmlb_layers kernels one replay re-runs (fused model layers)
+        self.fused = ()           # names of the models whose forward and backward ran fused in the capture
         self.replays = 0
         self.drop()
 
@@ -320,6 +328,8 @@ class _CapturedStep:
 
 class GraphedTrainStep(_CapturedStep):
     MODE = 'cuda_graph'
+    layer_plans = {}         # {model name: layers.CnnPlan} of the models whose layers run fused (set per instance)
+    _fused_ran = frozenset()  # names of the models that ran fused in the latest `_one_step`
 
     def __init__(self, stage):
         super().__init__(stage)
@@ -368,6 +378,18 @@ class GraphedTrainStep(_CapturedStep):
         self.flat_steps = 0
         self.exchanges = 0  # fused step exchanges with a metric descriptor == the device counter's value
         self.kernels_in_graph = 0
+        # models whose layers run fused (layers.py): plans made once, forwards swapped inside `_one_step` only
+        self.layer_plans = {}
+        if stage.fused_layers:
+            from .layers import plan_of
+
+            for name, m in pipeline.models.items():
+                plan, _ = plan_of(m.module if isinstance(m, DistributedDataParallel) else m)
+                if plan is not None and all(any(p is q for q in self.bucket.params) for p in plan.params):
+                    self.layer_plans[name] = plan
+        self.fused_models = []            # of the first captured signature
+        self.layer_kernels_in_graph = 0   # libdmlb_layers launches per replay of the first captured signature
+        self._fused_ran = set()
         # fused step exchange state, shared by every signature and by the flat step (created once, before the first step)
         self.ring = None
         self.feed = None
@@ -492,9 +514,17 @@ class GraphedTrainStep(_CapturedStep):
             ctxs = [m.no_sync() for m in self.ddp_models]  # the Reducer stays out of it: we synchronise the flat bucket
             for c in ctxs:
                 c.__enter__()
+            self._fused_ran = set()
             try:
-                loss = stage.train_step(batch)
-                loss.backward()
+                if self.layer_plans:
+                    from .layers import fused_forward
+
+                    with fused_forward(self.layer_plans, self.bucket, self._fused_ran):
+                        loss = stage.train_step(batch)
+                        loss.backward()
+                else:
+                    loss = stage.train_step(batch)
+                    loss.backward()
             finally:
                 for c in reversed(ctxs):
                     c.__exit__(None, None, None)
@@ -573,7 +603,10 @@ class GraphedTrainStep(_CapturedStep):
         return self.feed  # from now on python scalars of the feed's cells wait for the next exchange
 
     def _record(self, shape):
+        before = L.launch_count() if self.layer_plans else 0
         shape.loss, shape.step_metrics, shape.live_names, shape.keep = self._one_step(shape.batch, eager=False)
+        shape.layer_kernels = L.launch_count() - before if self.layer_plans else 0
+        shape.fused = tuple(sorted(self._fused_ran))
 
     def _capture(self, key, batch, leaves):
         shape = super()._capture(key, batch, leaves)
@@ -581,6 +614,8 @@ class GraphedTrainStep(_CapturedStep):
             self.first = shape
         if shape is self.first:
             self.kernels_in_graph = shape.kernels
+            self.layer_kernels_in_graph = shape.layer_kernels
+            self.fused_models = list(shape.fused)
         elif shape.kernels != self.first.kernels:
             self._say(('kernels', key), f'cuda_graph mode: the graph of batch signature {key} re-runs {shape.kernels} '
                                         f'libdmlb kernels per replay, the first graph {self.first.kernels}')

@@ -186,6 +186,10 @@ class TrainValStage(Stage):
         self.cuda_graph = False
         self.cuda_graph_warmup = 3
         self.cuda_graph_max_shapes = 4
+        # Extension: inside the captured training step (and its uncaptured flat step) a registered model of the small
+        # Conv3x3/ReLU/MaxPool -> Linear family runs under bf16 autocast as one forward and one backward kernel of
+        # libdmlb_layers.so instead of ~50 cuDNN / ATen kernels (layers.py).  False: the model's own kernels, always.
+        self.fused_layers = True
         self._graph = None
         self._eager_steps = 0
         # Extension: replay the validation step from CUDA graphs too (graphstep.GraphedValStep): one graph per batch
