@@ -32,6 +32,11 @@ class Seg(Structure):
     _fields_ = [('ptr', c_void_p), ('offset', c_int64), ('numel', c_int64)]
 
 
+class EmaSeg(Structure):
+    """dmlb_ema_seg: one run of an averaged model and its source (dmlb_ema_update)."""
+    _fields_ = [('avg', c_void_p), ('src', c_void_p), ('numel', c_int64), ('dtype', c_int32), ('_pad', c_int32)]
+
+
 class FoldEntry(Structure):
     _fields_ = [('src', c_void_p), ('imm', c_int64), ('src_dtype', c_int32), ('cell', c_int32), ('lanes', c_int32),
                 ('k', c_int32), ('steps', c_int32), ('_pad', c_int32)]
@@ -91,6 +96,7 @@ SIGNATURES = {
                                    c_int, c_void_p]),
     'dmlb_sgd_step_f32': (c_int, [c_void_p, c_void_p, c_void_p, c_size_t, c_double, c_double, c_double, c_double, c_int,
                                   c_int, c_void_p, c_float, c_void_p, c_int, c_void_p, c_int, c_void_p]),
+    'dmlb_ema_update': (c_int, [c_void_p, c_int, c_int64, c_void_p, c_void_p, c_int64, c_double, c_void_p]),
     'dmlb_multi_pack': (c_int, [c_void_p, c_int, c_int64, c_void_p, c_int, c_float, c_void_p]),
     'dmlb_multi_unpack': (c_int, [c_void_p, c_int, c_int64, c_void_p, c_int, c_float, c_void_p, c_void_p]),
     'dmlb_ipc_get_handle': (c_int, [c_void_p, c_void_p]),

@@ -10,35 +10,17 @@ static_assert(sizeof(cudaIpcMemHandle_t) == DMLB_IPC_HANDLE_BYTES, "IPC handle s
 
 namespace dmlb {
 
-constexpr int kChunk = 4096;  // elements one CTA moves per step in the multi-tensor kernels (16 KB of fp32)
-
-// Each CTA walks (segment, chunk) pairs: segments are found by a linear scan over the (small, L1-resident) table;
-// MNIST has 6 segments, ResNet-18 62.  Within a chunk the access is 128-bit when the segment base and the flat offset
-// are both vector-aligned (torch allocations are 512-B aligned; only odd-sized neighbours break flat alignment), else
-// scalar for that chunk.
+// The (segment, chunk) walk of for_each_seg_chunk.  Within a chunk the access is 128-bit when the segment base and the
+// flat offset are both vector-aligned (torch allocations are 512-B aligned; only odd-sized neighbours break flat
+// alignment), else scalar for that chunk.
 template <int kWire, bool kPack, bool kSumsq>
 __global__ void __launch_bounds__(kThreads, 2)
 multi_tensor_kernel(const dmlb_seg *__restrict__ segs, int count, long long n_chunks_total, void *flat, float scale,
                     double *sumsq_out) {
     double part = 0.0;
-    for (long long c = blockIdx.x; c < n_chunks_total; c += gridDim.x) {
-        // locate the segment owning global chunk c
-        long long acc = 0;
-        int s = 0;
-        long long local = 0;
-        for (; s < count; ++s) {
-            long long nc = (segs[s].numel + kChunk - 1) / kChunk;
-            if (c < acc + nc) {
-                local = c - acc;
-                break;
-            }
-            acc += nc;
-        }
-        if (s >= count) break;
-        const long long e0 = local * kChunk;
-        const long long len = min((long long)kChunk, segs[s].numel - e0);
-        float *g = segs[s].ptr + e0;
-        const long long off = segs[s].offset + e0;
+    for_each_seg_chunk(segs, count, n_chunks_total, [&](const dmlb_seg &seg, long long e0, long long len) {
+        float *g = seg.ptr + e0;
+        const long long off = seg.offset + e0;
         if (kWire == DMLB_WIRE_BF16) {
             uint16_t *w = reinterpret_cast<uint16_t *>(flat) + off;
             const bool vec = (((uintptr_t)g & 15) == 0) && (((uintptr_t)w & 7) == 0);
@@ -106,16 +88,11 @@ multi_tensor_kernel(const dmlb_seg *__restrict__ segs, int count, long long n_ch
                 }
             }
         }
-    }
+    });
     if (kSumsq) {
         double tot = block_sum(part);
         if (threadIdx.x == 0 && tot != 0.0) atomicAdd(sumsq_out, tot);
     }
-}
-
-static long long total_chunks_upper(int count, long long total) {
-    // every segment wastes at most one partial chunk
-    return (total + kChunk - 1) / kChunk + count;
 }
 
 }  // namespace dmlb

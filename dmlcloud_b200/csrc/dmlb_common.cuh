@@ -98,6 +98,36 @@ __device__ __forceinline__ double block_sum(double v) {
     return t;
 }
 
+// ---- multi-tensor walk ----------------------------------------------------------------------------------------------
+constexpr int kChunk = 4096;  // elements one CTA moves per step in the multi-tensor kernels (16 KB of fp32)
+
+// Each CTA walks (segment, chunk) pairs: segments are found by a linear scan over the (small, L1-resident) table;
+// MNIST has 6 segments, ResNet-18 62 (122 for a model EMA with its buffers).  `f(seg, e0, len)` handles elements
+// [e0, e0 + len) of segment `seg`; every chunk is handled by one whole CTA.  `Seg` is any table entry with a `numel`.
+template <class Seg, class F>
+__device__ __forceinline__ void for_each_seg_chunk(const Seg *__restrict__ segs, int count, long long n_chunks_total,
+                                                   F &&f) {
+    for (long long c = blockIdx.x; c < n_chunks_total; c += gridDim.x) {
+        long long acc = 0;
+        int s = 0;
+        long long local = 0;
+        for (; s < count; ++s) {
+            long long nc = (segs[s].numel + kChunk - 1) / kChunk;
+            if (c < acc + nc) {
+                local = c - acc;
+                break;
+            }
+            acc += nc;
+        }
+        if (s >= count) break;
+        const long long e0 = local * kChunk;
+        f(segs[s], e0, min((long long)kChunk, segs[s].numel - e0));
+    }
+}
+
+// chunks of a table of `count` segments holding `total` elements: every segment wastes at most one partial chunk
+inline long long total_chunks_upper(int count, long long total) { return (total + kChunk - 1) / kChunk + count; }
+
 // Grid for a grid-stride streaming kernel over `nvec` vector items, `per_thread` items per thread per sweep.
 // Small inputs: one CTA per sweep-chunk.  Large inputs: at most sm_count * ctas_per_sm resident CTAs, and the count is
 // chosen so that the number of sweeps is (almost) an integer — a plain "min(want, cap)" leaves the last sweep

@@ -218,6 +218,64 @@ sgd_kernel(float *__restrict__ param, float *__restrict__ grad, float *__restric
     }
 }
 
+// Model EMA (torchvision's ExponentialMovingAverage: AveragedModel with avg_fn = decay * avg + (1 - decay) * param and
+// use_buffers=True) over every parameter and buffer of one averaged model, walked as a segment table.  12 B/el when
+// averaging, 8 B/el when copying, ~0 when the launch is gated off by `every`.
+__device__ __forceinline__ float ema_f32(float avg, float src, float d, float e, bool copy) {
+    return copy ? src : __fadd_rn(__fmul_rn(d, avg), __fmul_rn(e, src));  // torch's two products and one sum, no FMA
+}
+
+__global__ void __launch_bounds__(kThreads, 2)
+ema_kernel(const dmlb_ema_seg *__restrict__ segs, int count, long long n_chunks_total, int64_t *n_averaged,
+           dmlb_ema_state *state, long long every, float d, float e) {
+    __shared__ int s_update, s_copy;
+    if (threadIdx.x == 0) {
+        s_update = (state->batch_index % every) == 0;
+        s_copy = *n_averaged == 0;
+    }
+    __syncthreads();
+    const bool copy = s_copy != 0;
+    if (s_update) {
+        for_each_seg_chunk(segs, count, n_chunks_total, [&](const dmlb_ema_seg &seg, long long e0, long long len) {
+            if (seg.dtype == DMLB_I64) {  // BatchNorm's num_batches_tracked: fp32 arithmetic, truncated back (copy_)
+                int64_t *a = reinterpret_cast<int64_t *>(seg.avg) + e0;
+                const int64_t *b = reinterpret_cast<const int64_t *>(seg.src) + e0;
+                for (long long i = threadIdx.x; i < len; i += kThreads)
+                    a[i] = copy ? b[i] : (int64_t)ema_f32((float)a[i], (float)b[i], d, e, false);
+                return;
+            }
+            float *a = reinterpret_cast<float *>(seg.avg) + e0;
+            const float *b = reinterpret_cast<const float *>(seg.src) + e0;
+            const bool vec = ((((uintptr_t)a | (uintptr_t)b) & 15) == 0);
+            const long long nv = vec ? len / 4 : 0;
+            for (long long i = threadIdx.x; i < nv; i += kThreads) {
+                const float4 s = reinterpret_cast<const float4 *>(b)[i];
+                float4 v;
+                if (copy) {
+                    v = s;
+                } else {
+                    v = reinterpret_cast<const float4 *>(a)[i];
+                    v.x = ema_f32(v.x, s.x, d, e, false), v.y = ema_f32(v.y, s.y, d, e, false);
+                    v.z = ema_f32(v.z, s.z, d, e, false), v.w = ema_f32(v.w, s.w, d, e, false);
+                }
+                reinterpret_cast<float4 *>(a)[i] = v;
+            }
+            for (long long i = nv * 4 + threadIdx.x; i < len; i += kThreads) a[i] = ema_f32(copy ? 0.0f : a[i], b[i], d, e, copy);
+        });
+    }
+    // every CTA has read batch_index and n_averaged by the time the last one arrives here
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        __threadfence();
+        const unsigned int done = atomicAdd(&state->done, 1u);
+        if (done == gridDim.x - 1) {
+            if (s_update) *n_averaged = state->hold ? 0 : *n_averaged + 1;
+            state->batch_index += 1;
+            state->done = 0u;
+        }
+    }
+}
+
 }  // namespace dmlb
 
 using namespace dmlb;
@@ -269,6 +327,18 @@ int dmlb_sgd_step_f32(float *param, float *grad, float *momentum_buf, size_t n, 
         const int grid = stream_grid(n, 1, 2);
         sgd_kernel<1><<<grid, kThreads, 0, st>>>(param, grad, momentum_buf, n, a, state, sumsq, lr_dev);
     }
+    return launched();
+}
+
+int dmlb_ema_update(const dmlb_ema_seg *segs, int count, int64_t total, int64_t *n_averaged, dmlb_ema_state *state,
+                    int64_t every, double decay, void *stream) {
+    if (!segs || !n_averaged || !state || count <= 0 || total < 0 || every < 1) return DMLB_EINVAL;
+    if ((((uintptr_t)segs | (uintptr_t)n_averaged | (uintptr_t)state)) & 7) return DMLB_EALIGN;
+    const long long chunks = total_chunks_upper(count, total);
+    const long long cap = (long long)sm_count() * 2;
+    const int grid = (int)(chunks < cap ? chunks : cap);
+    ema_kernel<<<grid, kThreads, 0, (cudaStream_t)stream>>>(segs, count, chunks, n_averaged, state, every, (float)decay,
+                                                            (float)(1.0 - decay));
     return launched();
 }
 

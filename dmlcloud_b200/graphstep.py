@@ -61,6 +61,7 @@ from torch.utils._pytree import tree_flatten, tree_unflatten
 
 from . import _layers as L
 from . import _native as N
+from .ema import registered
 from .gradsync import WIRES, PeerComm, wire_bytes
 from .metrics import HostFeed, StepRing, _RingResult
 
@@ -338,6 +339,7 @@ class GraphedTrainStep(_CapturedStep):
         self.world = dist.get_world_size()
         self.models = list(pipeline.models.values())
         self.ddp_models = [m for m in self.models if isinstance(m, DistributedDataParallel)]
+        self.emas = registered(pipeline.models)  # updated after the optimizers: one libdmlb node each per replay
         params, seen, groups = [], set(), 0
         for opt in stage.optimizers():
             device_lr = getattr(opt, 'device_lr', False)
@@ -499,6 +501,8 @@ class GraphedTrainStep(_CapturedStep):
                                                           self.sumsq.data_ptr(), self.clip, N.stream_ptr()), 'clip')
                     clip = None
                 opt.step()
+        for ema in self.emas:
+            ema.update_parameters()
 
     def _one_step(self, batch, eager):
         """One training step on `batch` (captured, or run as it is when `eager`): (loss, step metrics descriptor, live

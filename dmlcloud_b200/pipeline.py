@@ -25,6 +25,7 @@ import torch.distributed as dist
 from torch.nn.parallel import DistributedDataParallel
 
 from .checkpoint import CheckpointDir, find_slurm_checkpoint, generate_checkpoint_path
+from .ema import ExponentialMovingAverage
 from .metrics import MetricTracker, Reduction
 from .stage import Stage
 from .util.config import Conf
@@ -89,6 +90,8 @@ class TrainingPipeline:
                        best_metric: str = 'val/loss', verbose: bool = True, *, grad_wire: Optional[str] = None):
         if name in self.models:
             raise ValueError(f'Model with name {name} already exists')
+        if isinstance(model, ExponentialMovingAverage):
+            use_ddp = False  # its parameters take no gradient (DDP would refuse it); the stage updates it after the step
         model = model.to(self.device)  # move first, convert BN second: SyncBN conversion wants device-resident stats
         if sync_bn:
             model = self._convert_sync_bn(model)

@@ -24,6 +24,7 @@ from typing import Any, Dict, List, Optional, Union
 
 import torch
 
+from .ema import registered
 from .metrics import MetricTracker, Reduction
 from .util.distributed import is_root
 from .util.logging import DevNullIO, flush_log_handlers
@@ -285,6 +286,8 @@ class TrainValStage(Stage):
             self.clip_gradients()
         for opt in self.optimizers():
             opt.step()
+        for ema in registered(self.pipeline.models):
+            ema.update_parameters()  # after the optimizers, as torchvision's train_one_epoch does
 
     def _graphed_step(self, batch):
         """True if this batch was consumed by the captured step; False while still warming up eagerly."""
@@ -317,6 +320,8 @@ class TrainValStage(Stage):
         if hasattr(sampler, 'set_epoch'):
             sampler.set_epoch(self.current_epoch)
 
+        for ema in registered(self.pipeline.models):
+            ema.begin_epoch(self.current_epoch)  # every training step of the epoch, of any kind, counts as a batch
         slab = self.tracker._slab_or_create()
         if self.manual_gc:
             import gc

@@ -155,6 +155,39 @@ int dmlb_sgd_step_f32(float *param, float *grad, float *momentum_buf, size_t n, 
                       float max_norm, dmlb_adam_state *state, int advance, const double *lr_dev, int zero_grad,
                       void *stream);
 
+/* Model EMA: torchvision's ExponentialMovingAverage (torch.optim.swa_utils.AveragedModel with
+ * avg_fn = decay * avg + (1 - decay) * param, use_buffers=True; its `update_parameters` in the classification recipe's
+ * train_one_epoch) over every parameter and buffer of ONE averaged model in one launch.  `segs` is a DEVICE table of
+ * `count` segments built once on the host; `total` is the sum of their numel.  A segment pairs `avg` with `src` element
+ * by element in memory order, so both must be dense runs laid out alike; fp32 (DMLB_F32) or int64 (DMLB_I64) only.
+ * With d = fl32(decay), e = fl32(1 - decay) (1 - decay formed in fp64):
+ *   gated off      : state->batch_index % every != 0: nothing is read or written but the state
+ *   copy           : *n_averaged == 0: avg = src, bit for bit
+ *   fp32 average   : avg = fl32(fl32(d avg) + fl32(e src)), each product and the sum rounded once (no FMA); NaN and Inf
+ *                    propagate
+ *   int64 average  : the same in fp32 on float(avg) and float(src), truncated toward zero (torch's copy_ of the fp32
+ *                    result into the int64 buffer)
+ * The last CTA out advances state->batch_index, and on an updating launch sets *n_averaged = state->hold ? 0 :
+ * *n_averaged + 1 (torchvision resets n_averaged during LR warm-up).  No host sync, no allocation, deterministic and
+ * capturable.  `n_averaged` is the AveragedModel's own int64 buffer; `state` a 16-byte zero-initialised DEVICE block
+ * whose batch_index and hold the host sets at every epoch start.  Traffic: 12 B/el averaging, 8 B/el copying.
+ * DMLB_EINVAL: NULL pointers, count <= 0, total < 0, every < 1.  DMLB_EALIGN: segs, n_averaged or state not 8-byte
+ * aligned.  128-bit accesses where a chunk's avg and src are both 16-byte aligned, scalar otherwise. */
+typedef struct {
+    void *avg;
+    const void *src;
+    int64_t numel;
+    int32_t dtype; /* DMLB_F32 or DMLB_I64 */
+    int32_t _pad;
+} dmlb_ema_seg;
+typedef struct {
+    int64_t batch_index; /* training steps since the epoch began (torchvision's `i`)      */
+    int32_t hold;        /* != 0: every update leaves n_averaged at 0 (LR warm-up epochs) */
+    uint32_t done;       /* internal: CTAs that have finished the current launch          */
+} dmlb_ema_state;
+int dmlb_ema_update(const dmlb_ema_seg *segs, int count, int64_t total, int64_t *n_averaged, dmlb_ema_state *state,
+                    int64_t every, double decay, void *stream);
+
 /* Multi-tensor variants: gather `count` parameter gradients straight into / out of one flat wire buffer (the graph-
  * captured step keeps no DDP Reducer).  `segs` is a DEVICE array of dmlb_seg built once at registration. */
 typedef struct {
