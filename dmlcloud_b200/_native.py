@@ -143,6 +143,8 @@ SIGNATURES = {
                                c_int, c_void_p, c_void_p]),
     'dmlb_image_trivial_augment': (c_int, [c_void_p, c_void_p, c_int64, c_int32, c_int32, c_int32, c_int,
                                            POINTER(ImageNorm), c_void_p, c_int, c_int, c_void_p]),
+    'dmlb_image_auto_augment': (c_int, [c_void_p, c_void_p, c_void_p, c_int32, c_int64, c_int32, c_int32, c_int32, c_int,
+                                        POINTER(ImageNorm), c_void_p, c_int, c_int, c_void_p]),
 }
 
 _lib = None

@@ -682,14 +682,17 @@ static int launch_mix(dim3 grid, cudaStream_t st, const MixArgs &a) {
     return launched();
 }
 
-// ---- TrivialAugmentWide: one op per sample, then normalise (dmlb_image_trivial_augment) -----------------------------
-// (include/dmlb.h states the rule.)  One thread-block cluster per sample; CTA r of a cluster of n writes elements
-// [r S / n, (r + 1) S / n) of the sample's output in memory order (image_store_run).  Contrast, AutoContrast and
-// Equalize first reduce their statistics over pixels [r P / n, (r + 1) P / n) into the CTA's shared memory (a 128-bit
-// integer sum, per-channel min / max, per-channel 256-bin histograms), then every CTA folds the cluster's partials in
-// rank order through distributed shared memory between two cluster.sync(): exact integer and min / max folds, so the
-// result does not depend on the launch geometry.  Every CTA of a cluster holds the same sample, so the branch into
-// that phase is uniform.  Geometric ops and Sharpness gather from the sample, which sits in L2 at these sizes.
+// ---- Op chains: TrivialAugmentWide, RandAugment, AutoAugment, then normalise (dmlb_image_trivial_augment, ------------
+// dmlb_image_auto_augment; include/dmlb.h states the rule).  One thread-block cluster per sample; CTA r of a cluster
+// of n writes elements [r S / n, (r + 1) S / n) of each of the sample's outputs in memory order (image_store_run).
+// Contrast, AutoContrast and Equalize first reduce their statistics over pixels [r P / n, (r + 1) P / n) into the
+// CTA's shared memory (a 128-bit integer sum, per-channel min / max, per-channel 256-bin histograms), then every CTA
+// folds the cluster's partials in rank order through distributed shared memory between two cluster.sync(): exact
+// integer and min / max folds, so the result does not depend on the launch geometry.  Every CTA of a cluster holds the
+// same sample and the same op chain, so every branch on the op and every cluster.sync() is uniform.  Geometric ops and
+// Sharpness gather from the sample, which sits in L2 at these sizes.  A chain's slots but the last write their fp32
+// result into a work buffer (ping-pong between two when there are three or more), and the next slot reads it after a
+// cluster.sync(); an Identity slot is skipped, so the sample stays in its current buffer.
 
 namespace cg = cooperative_groups;
 
@@ -700,14 +703,17 @@ constexpr int kTaPixelsPerCta = 4096;         // cluster size = ceil(h w / this)
 constexpr int kTaMaxSide = 32768;             // h, w
 constexpr long long kTaMaxPixels = 1LL << 24; // h w: C h w fits an int run, the contrast sum fits 120 bits
 constexpr long long kTaMaxBatch = (1LL << 31) / kTaMaxCluster - 1;  // the grid is batch * cluster CTAs
+constexpr int kTaMaxChain = 4;                // ops per sample of dmlb_image_auto_augment
 enum { kTaIdentity, kTaShearX, kTaShearY, kTaTranslateX, kTaTranslateY, kTaRotate, kTaBrightness, kTaColor,
-       kTaContrast, kTaSharpness, kTaPosterize, kTaSolarize, kTaAutoContrast, kTaEqualize, kTaOps };
+       kTaContrast, kTaSharpness, kTaPosterize, kTaSolarize, kTaAutoContrast, kTaEqualize, kTaOps, kTaInvert = kTaOps };
 
 struct TaArgs {
     const float *src;
+    float *work;  // min(n_ops - 1, 2) fp32 batches: the results of a chain's inner slots (NULL when n_ops == 1)
     const int *ops;
     void *out;
-    long long S;  // C h w
+    long long S, batch;  // S = C h w
+    int n_ops, n_codes;  // ops per sample; op codes below n_codes are valid (14: TrivialAugment's, 15: with Invert)
     int C, h, w, nhwc, bilinear;
     float mean[4], std[4];
 };
@@ -753,8 +759,12 @@ __device__ __forceinline__ int ta_quantize(float v) {
     return t >= 255.0f ? 255 : (t > 0.0f ? (int)t : 0);
 }
 
-// One sample: its op and the per-sample constants, value(e) of output element e.
-template <bool kBf16>
+// One op of one sample: the op's constants, value(e) of output element e.  src is the sample's current buffer.
+// kWork: src is a work buffer that other CTAs of this cluster wrote earlier in this launch.  The non-coherent path
+// (__ldg, ld.global.nc) may serve such a read from a cache line filled before the write, so work is read through L2
+// (__ldcg), after the cluster.sync() whose release / acquire orders the writes before the reads.  The caller's src is
+// read-only for the whole launch (it overlaps neither work nor out), so it keeps the non-coherent path.
+template <bool kWork>
 struct TaSample {
     const float *src;
     const TaShared *s;
@@ -764,7 +774,9 @@ struct TaSample {
 
     __device__ __forceinline__ float in(int c, int y, int x) const {
         const int p = y * w + x;
-        return __ldg(src + (nhwc ? (long long)p * C + c : (long long)c * P + p));
+        const float *q = src + (nhwc ? (long long)p * C + c : (long long)c * P + p);
+        if constexpr (kWork) return __ldcg(q);
+        return __ldg(q);
     }
     __device__ __forceinline__ float tap(int c, int y, int x) const {
         return (unsigned)y < (unsigned)h && (unsigned)x < (unsigned)w ? in(c, y, x) : 0.0f;
@@ -833,9 +845,12 @@ struct TaSample {
             }
             case kTaAutoContrast: return ta_clamp01(__fdiv_rn(__fsub_rn(in(c, y, x), s->cmin[c]), s->cinv[c]));
             case kTaEqualize: return s->lut[c][ta_quantize(in(c, y, x))];
+            case kTaInvert: return __fsub_rn(1.0f, in(c, y, x));
             default: return geometric(c, y, x);
         }
     }
+    // kNorm: normalised into kBf16 | fp32 bits (the chain's last slot), else the fp32 bits of the op's value
+    template <bool kBf16, bool kNorm>
     __device__ __forceinline__ uint32_t value(long long e) const {
         int c, p;
         if (nhwc) {
@@ -845,21 +860,22 @@ struct TaSample {
         }
         if (nan) return kBf16 ? 0x7fc0u : 0x7fc00000u;
         const int y = p / w;
-        const float v = __fdiv_rn(__fsub_rn(op_value(c, y, p - y * w), mean[c]), std[c]);
+        float v = op_value(c, y, p - y * w);
+        if (kNorm) v = __fdiv_rn(__fsub_rn(v, mean[c]), std[c]);
         return kBf16 ? (uint32_t)f32_to_bf16(v) : __float_as_uint(v);
     }
 };
 
-template <bool kBf16>
+template <bool kWork, bool kBf16, bool kNorm>
 struct TaCursor {
-    const TaSample<kBf16> &s;
+    const TaSample<kWork> &s;
     long long e;
-    __device__ __forceinline__ uint32_t next() { return s.value(e++); }
+    __device__ __forceinline__ uint32_t next() { return s.template value<kBf16, kNorm>(e++); }
 };
 
 // The cluster's statistics of the sample's op (Contrast, AutoContrast, Equalize) into s; every CTA calls it.
-template <bool kBf16>
-__device__ void ta_statistics(const TaSample<kBf16> &t, TaShared &s, cg::cluster_group &cluster) {
+template <bool kWork>
+__device__ void ta_statistics(const TaSample<kWork> &t, TaShared &s, cg::cluster_group &cluster) {
     const int rank = (int)cluster.block_rank(), n = (int)cluster.num_blocks();
     const int p0 = (int)((long long)t.P * rank / n), p1 = (int)((long long)t.P * (rank + 1) / n);
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
@@ -950,15 +966,22 @@ __device__ void ta_statistics(const TaSample<kBf16> &t, TaShared &s, cg::cluster
     __syncthreads();
 }
 
-template <bool kBf16>
-__global__ void __launch_bounds__(kTaThreads) image_trivial_augment_kernel(const TaArgs a) {
-    __shared__ TaShared s;
-    cg::cluster_group cluster = cg::this_cluster();
-    const int n = (int)cluster.num_blocks(), rank = (int)cluster.block_rank();
-    const long long i = blockIdx.x / n;
-    const int *row = a.ops + 8 * i;
-    TaSample<kBf16> t;
-    t.src = a.src + i * a.S;
+// Whether op row `row` makes its sample NaN: an op code outside [0, n_codes), or a Posterize magnitude outside (-1, 9).
+__device__ __forceinline__ bool ta_bad_row(const int *row, int n_codes) {
+    const int op = __ldg(row);
+    const float mag = __int_as_float(__ldg(row + 1));
+    return op < 0 || op >= n_codes || (op == kTaPosterize && !(mag > -1.0f && mag < 9.0f));
+}
+
+// One slot of a sample: the op of `row` on the sample's current buffer `cur`; the sample's elements [e0, e1) are
+// written to dst from its element `first` on (kNorm: normalised into out's dtype, else fp32).  Every CTA of the
+// cluster calls it.
+template <bool kWork, bool kBf16, bool kNorm>
+__device__ __forceinline__ void ta_slot(const TaArgs &a, TaShared &s, cg::cluster_group &cluster, const int *row,
+                                        const float *cur, bool nan, void *dst, long long first, long long e0,
+                                        long long e1) {
+    TaSample<kWork> t;
+    t.src = cur;
     t.s = &s;
     t.mean = a.mean, t.std = a.std;
     t.C = a.C, t.h = a.h, t.w = a.w, t.P = a.h * a.w, t.nhwc = a.nhwc, t.bilinear = a.bilinear;
@@ -973,11 +996,45 @@ __global__ void __launch_bounds__(kTaThreads) image_trivial_augment_kernel(const
         if (deg < 0.0) deg += 360.0;
         t.rot = deg == 0.0 ? 4 : deg == 180.0 ? 2 : a.h != a.w ? 0 : deg == 90.0 ? 1 : deg == 270.0 ? 3 : 0;
     }
-    t.nan = t.op < 0 || t.op >= kTaOps || __ldg(t.src) != __ldg(t.src) ||
-            (t.op == kTaPosterize && !(t.mag > -1.0f && t.mag < 9.0f));
+    t.nan = nan;
     if (!t.nan && (t.op == kTaContrast || t.op == kTaAutoContrast || t.op == kTaEqualize)) ta_statistics(t, s, cluster);
+    image_store_run<kBf16>(dst, first, (int)(e1 - e0), [&](int k) { return TaCursor<kWork, kBf16, kNorm>{t, e0 + k}; });
+}
+
+// kChain: n_ops may exceed 1 (dmlb_image_auto_augment); the one-op kernel (dmlb_image_trivial_augment, and n_ops == 1)
+// keeps only the last slot, which reads src through the non-coherent path.  The chain holds the state of every slot
+// kind at once: two CTAs per SM give ptxas the registers to keep it without spilling.
+template <bool kBf16, bool kChain>
+__global__ void __launch_bounds__(kTaThreads, kChain ? 2 : 0) image_augment_kernel(const TaArgs a) {
+    __shared__ TaShared s;
+    cg::cluster_group cluster = cg::this_cluster();
+    const int n = (int)cluster.num_blocks(), rank = (int)cluster.block_rank();
+    const long long i = blockIdx.x / n;
+    const int n_ops = kChain ? a.n_ops : 1;
+    const int *rows = a.ops + 8LL * n_ops * i;
+    const float *src = a.src + i * a.S;
+    bool nan = __ldg(src) != __ldg(src);
+    for (int k = 0; k < n_ops; ++k) nan = nan || ta_bad_row(rows + 8 * k, a.n_codes);
     const long long e0 = a.S * rank / n, e1 = a.S * (rank + 1) / n;
-    image_store_run<kBf16>(a.out, i * a.S + e0, (int)(e1 - e0), [&](int k) { return TaCursor<kBf16>{t, e0 + k}; });
+    int cur = -1;  // the sample's current buffer: src (-1) or work batch 0 / 1
+    for (int k = 0; k + 1 < n_ops && !nan; ++k) {
+        if (__ldg(rows + 8 * k) == kTaIdentity) continue;
+        const int next = cur == 0 ? 1 : 0;
+        float *dst = a.work + (next * a.batch + i) * a.S;
+        if (cur < 0)
+            ta_slot<false, false, false>(a, s, cluster, rows + 8 * k, src, false, dst, e0, e0, e1);
+        else
+            ta_slot<true, false, false>(a, s, cluster, rows + 8 * k, a.work + (cur * a.batch + i) * a.S, false, dst, e0,
+                                        e0, e1);
+        cluster.sync();  // every CTA's part of dst is written and visible to the cluster (release / acquire)
+        cur = next;
+    }
+    const int *last = rows + 8 * (n_ops - 1);
+    if (!kChain || cur < 0)
+        ta_slot<false, kBf16, true>(a, s, cluster, last, src, nan, a.out, i * a.S + e0, e0, e1);
+    else
+        ta_slot<true, kBf16, true>(a, s, cluster, last, a.work + (cur * a.batch + i) * a.S, nan, a.out, i * a.S + e0, e0,
+                                   e1);
 }
 
 static int ta_cluster(long long pixels) {
@@ -985,10 +1042,10 @@ static int ta_cluster(long long pixels) {
     return (int)(n < kTaMaxCluster ? n : kTaMaxCluster);
 }
 
-template <bool kBf16>
-static int launch_trivial_augment(long long batch, int cluster, cudaStream_t st, const TaArgs &a) {
+template <bool kBf16, bool kChain>
+static int launch_augment(int cluster, cudaStream_t st, const TaArgs &a) {
     cudaLaunchConfig_t cfg = {};
-    cfg.gridDim = dim3((unsigned)(batch * cluster));
+    cfg.gridDim = dim3((unsigned)(a.batch * cluster));
     cfg.blockDim = dim3(kTaThreads);
     cfg.stream = st;
     cudaLaunchAttribute attr;
@@ -996,9 +1053,49 @@ static int launch_trivial_augment(long long batch, int cluster, cudaStream_t st,
     attr.val.clusterDim.x = (unsigned)cluster, attr.val.clusterDim.y = 1, attr.val.clusterDim.z = 1;
     cfg.attrs = &attr;
     cfg.numAttrs = 1;
-    const cudaError_t e = cudaLaunchKernelEx(&cfg, image_trivial_augment_kernel<kBf16>, a);
+    const cudaError_t e = cudaLaunchKernelEx(&cfg, image_augment_kernel<kBf16, kChain>, a);
     const int r = launched();
     return e != cudaSuccess ? -(int)e : r;
+}
+
+static bool overlaps(const void *p, long long p_bytes, const void *q, long long q_bytes) {
+    const uintptr_t p0 = (uintptr_t)p, q0 = (uintptr_t)q;
+    return p_bytes > 0 && q_bytes > 0 && p0 < q0 + (uintptr_t)q_bytes && q0 < p0 + (uintptr_t)p_bytes;
+}
+
+// The checks and the launch of both op-chain entries (n_codes: 14 for TrivialAugment's ops, 15 with Invert).
+static int augment(const float *src, float *work, const int32_t *ops, int n_ops, int n_codes, int64_t batch, int32_t C,
+                   int32_t h, int32_t w, int bilinear, const dmlb_image_norm *norm, void *out, int out_bf16,
+                   int channels_last, void *stream) {
+    if (batch < 0 || batch > kTaMaxBatch || !norm || (C != 1 && C != 3) || h < 1 || w < 1 || h > kTaMaxSide ||
+        w > kTaMaxSide || (long long)h * w > kTaMaxPixels || (bilinear != 0 && bilinear != 1) || n_ops < 1 ||
+        n_ops > kTaMaxChain)
+        return DMLB_EINVAL;
+    TaArgs a;
+    if (!pack_norm(norm, C, a.mean, a.std)) return DMLB_EINVAL;
+    if (batch > 0 && (!src || !ops || !out || (n_ops > 1 && !work))) return DMLB_EINVAL;
+    const long long S = (long long)C * h * w;
+    const long long src_bytes = batch * S * 4, out_bytes = batch * S * (out_bf16 ? 2 : 4);
+    const long long work_bytes = n_ops > 1 ? (n_ops > 2 ? 2 : 1) * src_bytes : 0;
+    if (overlaps(src, src_bytes, out, out_bytes) || overlaps(work, work_bytes, src, src_bytes) ||
+        overlaps(work, work_bytes, ops, batch * n_ops * 32) || overlaps(work, work_bytes, out, out_bytes))
+        return DMLB_EINVAL;
+    if (((uintptr_t)src & 3) != 0 || ((uintptr_t)ops & 3) != 0 || ((uintptr_t)out & (out_bf16 ? 1 : 3)) != 0 ||
+        (n_ops > 1 && ((uintptr_t)work & 3) != 0))
+        return DMLB_EALIGN;
+    if (batch == 0) return DMLB_OK;
+
+    a.src = src;
+    a.work = n_ops > 1 ? work : nullptr;
+    a.ops = ops;
+    a.out = out;
+    a.S = S, a.batch = batch;
+    a.n_ops = n_ops, a.n_codes = n_codes;
+    a.C = C, a.h = h, a.w = w, a.nhwc = channels_last ? 1 : 0, a.bilinear = bilinear;
+    const int cluster = ta_cluster((long long)h * w);
+    cudaStream_t st = (cudaStream_t)stream;
+    if (n_ops > 1) return out_bf16 ? launch_augment<true, true>(cluster, st, a) : launch_augment<false, true>(cluster, st, a);
+    return out_bf16 ? launch_augment<true, false>(cluster, st, a) : launch_augment<false, false>(cluster, st, a);
 }
 
 }  // namespace dmlb
@@ -1165,28 +1262,14 @@ int dmlb_image_mix(const float *src, const int64_t *idx, const int64_t *labels, 
 int dmlb_image_trivial_augment(const float *src, const int32_t *ops, int64_t batch, int32_t C, int32_t h, int32_t w,
                                int bilinear, const dmlb_image_norm *norm, void *out, int out_bf16, int channels_last,
                                void *stream) {
-    if (batch < 0 || batch > kTaMaxBatch || !norm || (C != 1 && C != 3) || h < 1 || w < 1 || h > kTaMaxSide ||
-        w > kTaMaxSide || (long long)h * w > kTaMaxPixels || (bilinear != 0 && bilinear != 1))
-        return DMLB_EINVAL;
-    TaArgs a;
-    if (!pack_norm(norm, C, a.mean, a.std)) return DMLB_EINVAL;
-    if (batch > 0 && (!src || !ops || !out)) return DMLB_EINVAL;
-    const long long S = (long long)C * h * w;
-    const uintptr_t s0 = (uintptr_t)src, s1 = s0 + (uintptr_t)(batch * S * 4);
-    const uintptr_t o0 = (uintptr_t)out, o1 = o0 + (uintptr_t)(batch * S * (out_bf16 ? 2 : 4));
-    if (batch > 0 && s0 < o1 && o0 < s1) return DMLB_EINVAL;
-    if ((s0 & 3) != 0 || ((uintptr_t)ops & 3) != 0 || (o0 & (out_bf16 ? 1 : 3)) != 0) return DMLB_EALIGN;
-    if (batch == 0) return DMLB_OK;
+    return augment(src, nullptr, ops, 1, kTaOps, batch, C, h, w, bilinear, norm, out, out_bf16, channels_last, stream);
+}
 
-    a.src = src;
-    a.ops = ops;
-    a.out = out;
-    a.S = S;
-    a.C = C, a.h = h, a.w = w, a.nhwc = channels_last ? 1 : 0, a.bilinear = bilinear;
-    const int cluster = ta_cluster((long long)h * w);
-    cudaStream_t st = (cudaStream_t)stream;
-    return out_bf16 ? launch_trivial_augment<true>(batch, cluster, st, a)
-                    : launch_trivial_augment<false>(batch, cluster, st, a);
+int dmlb_image_auto_augment(const float *src, float *work, const int32_t *ops, int32_t n_ops, int64_t batch, int32_t C,
+                            int32_t h, int32_t w, int bilinear, const dmlb_image_norm *norm, void *out, int out_bf16,
+                            int channels_last, void *stream) {
+    return augment(src, work, ops, n_ops, kTaOps + 1, batch, C, h, w, bilinear, norm, out, out_bf16, channels_last,
+                   stream);
 }
 
 }  // extern "C"

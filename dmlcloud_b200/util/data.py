@@ -32,6 +32,10 @@ or device tables (one per epoch).  They all come from one counter hash:
                ratio from 34 + 3a, the offsets from 35 + 3a
       63       ta_ops: TrivialAugmentWide's op = below(word 63 >> 32, 14) and bin = below(word 63 & 0xffffffff, bins)
       64       ta_ops: a signed op's magnitude is negated when u53(word 64) <= 0.5
+      65..72   ra_ops: RandAugment's slot k (0..3) takes its op = below(word 65 + 2k >> 32, 14) and negates a signed
+               op's magnitude when u53(word 66 + 2k) <= 0.5
+      65..69   aa_ops: AutoAugment's sub-policy = below(word 65 >> 32, 25); its op k (0, 1) runs when
+               u53(word 66 + 2k) <= p_k and negates a signed op's magnitude when u53(word 67 + 2k) <= 0.5
   batch hash hb = mix(mix(e ^ (rank + g + 2^63)) ^ (batch + g)), e = mix(mix(seed + g) ^ (epoch + g)) (batch_hash); a
              row's hash is mix(e ^ (row + g)) with row < 2^63 and mix is a bijection, so hb is never a row's hash.
              mix_batch_params takes the MixUp / CutMix choice from mix(hb + g) >> 63, CutMix's centre from
@@ -313,7 +317,7 @@ class _DeviceImageBatches(DeviceShardedDataset):
     def __init__(self, images, labels, batch_size, mean, std, crop, hflip, memory_format, out_dtype, shuffle,
                  even_shards, seed, aug_seed, rank, world_size, device, drop_last, mixup_alpha, cutmix_alpha,
                  num_classes, random_erase, erase_scale, erase_ratio, erase_value, trivial_augment, ta_bins,
-                 ta_interpolation):
+                 ta_interpolation, auto_augment, ra_num_ops, ra_magnitude, ra_bins):
         if memory_format not in (torch.contiguous_format, torch.channels_last):
             raise ValueError('memory_format must be torch.contiguous_format or torch.channels_last')
         super().__init__(images, labels, batch_size, shuffle=shuffle, even_shards=even_shards, seed=seed, rank=rank,
@@ -359,18 +363,37 @@ class _DeviceImageBatches(DeviceShardedDataset):
             raise ValueError(f'crop {self.crop}: dmlb_image_mix takes sides of at most 32768')
         self.trivial_augment = bool(trivial_augment)
         self.ta_bins, self.ta_interpolation = int(ta_bins), ta_interpolation
-        if self.trivial_augment:
+        self.auto_augment = auto_augment
+        self.ra_num_ops, self.ra_magnitude, self.ra_bins = int(ra_num_ops), int(ra_magnitude), int(ra_bins)
+        if auto_augment is not None:
+            if self.trivial_augment:
+                raise ValueError('auto_augment and trivial_augment are two policies; torchvision applies one')
+            if auto_augment not in ('ra',) + tuple(AA_POLICIES):
+                raise ValueError(f"auto_augment must be None, 'ra', 'imagenet', 'cifar10' or 'svhn', got "
+                                 f"{auto_augment!r}")
+            if auto_augment == 'ra':
+                if not 0 <= self.ra_num_ops <= 4:
+                    raise ValueError(f'ra_num_ops must lie in 0..4, got {ra_num_ops}')
+                if self.ra_bins < 2:
+                    raise ValueError(f'ra_bins must be >= 2, got {ra_bins}')
+                if not 0 <= self.ra_magnitude < self.ra_bins:
+                    raise ValueError(f'ra_magnitude must lie in [0, ra_bins = {self.ra_bins}), got {ra_magnitude}')
+        # ops per sample: 1 (TrivialAugmentWide), ra_num_ops (RandAugment), 2 (AutoAugment) or 0 (none)
+        self._chain = 1 if self.trivial_augment else 0 if auto_augment is None else \
+            self.ra_num_ops if auto_augment == 'ra' else 2
+        if self.trivial_augment or auto_augment is not None:
+            name = 'TrivialAugmentWide' if self.trivial_augment else 'auto_augment'
             if C not in (1, 3):
-                raise ValueError(f'TrivialAugmentWide takes 1 or 3 channels, got {C}')
-            if self.ta_bins < 2:
+                raise ValueError(f'{name} takes 1 or 3 channels, got {C}')
+            if self.trivial_augment and self.ta_bins < 2:
                 raise ValueError(f'ta_bins must be >= 2, got {ta_bins}')
             if ta_interpolation not in ('nearest', 'bilinear'):
                 raise ValueError(f"ta_interpolation must be 'nearest' or 'bilinear', got {ta_interpolation!r}")
             h, w = self.crop
             if max(h, w) > 32768 or h * w > 1 << 24:
-                raise ValueError(f'crop {self.crop}: TrivialAugmentWide takes sides of at most 32768 and at most '
-                                 '2^24 pixels')
-            self._ta_magnitudes = ta_magnitudes(self.ta_bins)
+                raise ValueError(f'crop {self.crop}: {name} takes sides of at most 32768 and at most 2^24 pixels')
+            if self.trivial_augment:
+                self._ta_magnitudes = ta_magnitudes(self.ta_bins)
             self._identity = self._N.ImageNorm.of([0.0] * C, [1.0] * C)
 
     def _shard_rows(self):
@@ -392,15 +415,36 @@ class _DeviceImageBatches(DeviceShardedDataset):
         return ta_ops(self._shard_rows(), self.ta_bins, self.crop[0], self.crop[1], self.aug_seed, self.epoch,
                       self._ta_magnitudes)
 
+    def epoch_aa_ops(self):
+        """int32 [shard_len(), n_ops, 8] numpy op rows of this rank's samples this epoch, in iteration order:
+        ra_ops (n_ops = ra_num_ops) or aa_ops (n_ops = 2) of the auto_augment policy."""
+        h, w = self.crop
+        if self.auto_augment == 'ra':
+            return ra_ops(self._shard_rows(), self.ra_num_ops, self.ra_magnitude, self.ra_bins, h, w, self.aug_seed,
+                          self.epoch)
+        return aa_ops(self._shard_rows(), self.auto_augment, h, w, self.aug_seed, self.epoch)
+
     def _augment(self, ops, scratch, x):
-        """TrivialAugmentWide and the normalisation of the identity-normalised fp32 `scratch` into x (one launch)."""
+        """The op rows `ops` (TrivialAugmentWide's, or a chain of RandAugment's or AutoAugment's) and the normalisation
+        of the identity-normalised fp32 `scratch` into x (one launch)."""
         N = self._N
+        lib = N.cuda_lib(self.device.index)
         _, _, C = self.item_shape
         h, w = self.crop
-        N.check(N.cuda_lib(self.device.index).dmlb_image_trivial_augment(
-            scratch.data_ptr(), ops.data_ptr(), ops.shape[0], C, h, w, int(self.ta_interpolation == 'bilinear'),
-            self._norm, x.data_ptr(), int(x.dtype == torch.bfloat16), int(self.memory_format == torch.channels_last),
-            N.stream_ptr()), 'image_trivial_augment')
+        bilinear, bf16 = int(self.ta_interpolation == 'bilinear'), int(x.dtype == torch.bfloat16)
+        nhwc = int(self.memory_format == torch.channels_last)
+        if self.trivial_augment:
+            N.check(lib.dmlb_image_trivial_augment(scratch.data_ptr(), ops.data_ptr(), ops.shape[0], C, h, w, bilinear,
+                                                   self._norm, x.data_ptr(), bf16, nhwc, N.stream_ptr()),
+                    'image_trivial_augment')
+            return
+        b, n_ops = ops.shape[0], ops.shape[1]
+        work = None
+        if n_ops > 1:
+            work = torch.empty(min(n_ops - 1, 2) * scratch.numel(), dtype=torch.float32, device=self.device)
+        N.check(lib.dmlb_image_auto_augment(scratch.data_ptr(), None if work is None else work.data_ptr(),
+                                            ops.data_ptr(), n_ops, b, C, h, w, bilinear, self._norm, x.data_ptr(),
+                                            bf16, nhwc, N.stream_ptr()), 'image_auto_augment')
 
     def batch_params(self, batch):
         """{'mode', 'lam', 'lam_adjusted', 'box'} of this rank's batch number `batch` this epoch (mix_batch_params)."""
@@ -447,8 +491,8 @@ class _DeviceImageBatches(DeviceShardedDataset):
         return x, y
 
     def _images(self, view, rows, ops, x):
-        """The images of `view` into x: _launch alone, or (TrivialAugmentWide) _launch into an fp32 scratch batch with
-        the identity normalisation, which dmlb_image_trivial_augment augments and normalises into x."""
+        """The images of `view` into x: _launch alone, or (TrivialAugmentWide, auto_augment) _launch into an fp32
+        scratch batch with the identity normalisation, which _augment augments and normalises into x."""
         if ops is None:
             self._launch(view, rows, x, self._norm)
             return
@@ -469,6 +513,8 @@ class _DeviceImageBatches(DeviceShardedDataset):
             erase = torch.from_numpy(self.epoch_erase_boxes()).to(self.device)
         if self.trivial_augment:
             ops = torch.from_numpy(self.epoch_ta_ops()).to(self.device)
+        elif self._chain:
+            ops = torch.from_numpy(self.epoch_aa_ops()).to(self.device)
         for start in range(0, count, self.batch_size):
             b = min(self.batch_size, count - start)
             if b < self.batch_size and self.drop_last:
@@ -521,13 +567,24 @@ class DeviceImageDataset(_DeviceImageBatches):
                     1 or 3.  A sample's op and magnitude depend only on (aug_seed, epoch, dataset index) (ta_ops);
                     epoch_ta_ops() gives the epoch's table.  It adds one launch per batch: the image kernel writes an
                     fp32 scratch batch with mean 0 and std 1, which dmlb_image_trivial_augment augments and normalises.
+
+    RandAugment and AutoAugment (torchvision's `--auto-augment ra | imagenet | cifar10 | svhn`, off by default):
+      auto_augment  None, 'ra' (RandAugment(num_ops=ra_num_ops, magnitude=ra_magnitude,
+                    num_magnitude_bins=ra_bins)) or an AutoAugment policy ('imagenet', 'cifar10', 'svhn'), torchvision
+                    v2's with fill=None, at TrivialAugmentWide's place in the pipeline; not together with
+                    trivial_augment.  ta_interpolation is the interpolation of whichever policy is on.  ra_num_ops
+                    lies in 0..4 (0 leaves the batches as with auto_augment=None), ra_magnitude in [0, ra_bins).  The
+                    draws depend only on (aug_seed, epoch, dataset index) (ra_ops, aa_ops); epoch_aa_ops() gives the
+                    epoch's table.  Every chain is one launch (dmlb_image_auto_augment) in place of the
+                    TrivialAugmentWide launch, whatever ra_num_ops is.
     """
 
     def __init__(self, images, labels, batch_size, mean, std, crop=None, padding=0, random_crop=True, hflip=False,
                  memory_format=torch.contiguous_format, out_dtype=torch.float32, shuffle=True, even_shards=True, seed=0,
                  aug_seed=None, rank=None, world_size=None, device=None, drop_last=False, mixup_alpha=0.0,
                  cutmix_alpha=0.0, num_classes=None, random_erase=0.0, erase_scale=(0.02, 0.33), erase_ratio=(0.3, 3.3),
-                 erase_value=0.0, trivial_augment=False, ta_bins=31, ta_interpolation='nearest'):
+                 erase_value=0.0, trivial_augment=False, ta_bins=31, ta_interpolation='nearest', auto_augment=None,
+                 ra_num_ops=2, ra_magnitude=9, ra_bins=31):
         H, W, _ = _image_hwc(images)
         self.padding = int(padding)
         if crop is None:
@@ -539,7 +596,7 @@ class DeviceImageDataset(_DeviceImageBatches):
         super().__init__(images, labels, batch_size, mean, std, crop, hflip, memory_format, out_dtype, shuffle,
                          even_shards, seed, aug_seed, rank, world_size, device, drop_last, mixup_alpha, cutmix_alpha,
                          num_classes, random_erase, erase_scale, erase_ratio, erase_value, trivial_augment, ta_bins,
-                         ta_interpolation)
+                         ta_interpolation, auto_augment, ra_num_ops, ra_magnitude, ra_bins)
 
     def epoch_table(self):
         """int32 [shard_len(), 3] numpy {top, left, flipped} (crop_windows) of this rank's samples this epoch, in
@@ -728,8 +785,13 @@ def ta_ops(rows, bins, h, w, seed, epoch, magnitudes=None):
     op = _below(w63 >> np.uint64(32), 14)
     mag = mags[op, _below(w63 & np.uint64(0xFFFFFFFF), bins)].astype(np.float32)
     neg = _TA_SIGNED[op] & (_u53(hr, TA_WORD + 1) <= 0.5)
-    mag = np.where(neg, -mag, mag).astype(np.float32)
-    out = np.zeros((len(hr), 8), dtype=np.int32)
+    return _op_rows(op, np.where(neg, -mag, mag).astype(np.float32), h, w)
+
+
+def _op_rows(op, mag, h, w):
+    """int32 [len(op), 8] op rows {op, magnitude, theta0..5} of the int ops and fp32 magnitudes, theta the ta_theta of
+    the geometric ops, formed once per distinct (op, magnitude)."""
+    out = np.zeros((len(op), 8), dtype=np.int32)
     out[:, 0] = op
     out[:, 1] = mag.view(np.int32)
     geo = (op >= 1) & (op <= 5)
@@ -737,6 +799,103 @@ def ta_ops(rows, bins, h, w, seed, epoch, magnitudes=None):
         keys, inverse = np.unique(np.stack([op[geo], mag[geo].view(np.int32)], axis=1), axis=0, return_inverse=True)
         thetas = np.stack([ta_theta(int(o), float(np.int32(m).view(np.float32)), h, w) for o, m in keys])
         out[geo, 2:] = thetas[inverse.reshape(-1)].view(np.int32)
+    return out
+
+
+AA_WORD = 65  # the RandAugment and AutoAugment words of a row, 65..72, follow the TrivialAugmentWide words
+AA_OPS = TA_OPS + ('Invert',)  # op codes 0..14 of dmlb_image_auto_augment
+_AA_SIGNED = (np.arange(15) >= 1) & (np.arange(15) <= 9)
+AA_POLICIES = {  # torchvision's AutoAugmentPolicy sub-policies: ((op, probability, magnitude bin or None), x2)
+    'imagenet': (
+        (('Posterize', 0.4, 8), ('Rotate', 0.6, 9)), (('Solarize', 0.6, 5), ('AutoContrast', 0.6, None)),
+        (('Equalize', 0.8, None), ('Equalize', 0.6, None)), (('Posterize', 0.6, 7), ('Posterize', 0.6, 6)),
+        (('Equalize', 0.4, None), ('Solarize', 0.2, 4)), (('Equalize', 0.4, None), ('Rotate', 0.8, 8)),
+        (('Solarize', 0.6, 3), ('Equalize', 0.6, None)), (('Posterize', 0.8, 5), ('Equalize', 1.0, None)),
+        (('Rotate', 0.2, 3), ('Solarize', 0.6, 8)), (('Equalize', 0.6, None), ('Posterize', 0.4, 6)),
+        (('Rotate', 0.8, 8), ('Color', 0.4, 0)), (('Rotate', 0.4, 9), ('Equalize', 0.6, None)),
+        (('Equalize', 0.0, None), ('Equalize', 0.8, None)), (('Invert', 0.6, None), ('Equalize', 1.0, None)),
+        (('Color', 0.6, 4), ('Contrast', 1.0, 8)), (('Rotate', 0.8, 8), ('Color', 1.0, 2)),
+        (('Color', 0.8, 8), ('Solarize', 0.8, 7)), (('Sharpness', 0.4, 7), ('Invert', 0.6, None)),
+        (('ShearX', 0.6, 5), ('Equalize', 1.0, None)), (('Color', 0.4, 0), ('Equalize', 0.6, None)),
+        (('Equalize', 0.4, None), ('Solarize', 0.2, 4)), (('Solarize', 0.6, 5), ('AutoContrast', 0.6, None)),
+        (('Invert', 0.6, None), ('Equalize', 1.0, None)), (('Color', 0.6, 4), ('Contrast', 1.0, 8)),
+        (('Equalize', 0.8, None), ('Equalize', 0.6, None))),
+    'cifar10': (
+        (('Invert', 0.1, None), ('Contrast', 0.2, 6)), (('Rotate', 0.7, 2), ('TranslateX', 0.3, 9)),
+        (('Sharpness', 0.8, 1), ('Sharpness', 0.9, 3)), (('ShearY', 0.5, 8), ('TranslateY', 0.7, 9)),
+        (('AutoContrast', 0.5, None), ('Equalize', 0.9, None)), (('ShearY', 0.2, 7), ('Posterize', 0.3, 7)),
+        (('Color', 0.4, 3), ('Brightness', 0.6, 7)), (('Sharpness', 0.3, 9), ('Brightness', 0.7, 9)),
+        (('Equalize', 0.6, None), ('Equalize', 0.5, None)), (('Contrast', 0.6, 7), ('Sharpness', 0.6, 5)),
+        (('Color', 0.7, 7), ('TranslateX', 0.5, 8)), (('Equalize', 0.3, None), ('AutoContrast', 0.4, None)),
+        (('TranslateY', 0.4, 3), ('Sharpness', 0.2, 6)), (('Brightness', 0.9, 6), ('Color', 0.2, 8)),
+        (('Solarize', 0.5, 2), ('Invert', 0.0, None)), (('Equalize', 0.2, None), ('AutoContrast', 0.6, None)),
+        (('Equalize', 0.2, None), ('Equalize', 0.6, None)), (('Color', 0.9, 9), ('Equalize', 0.6, None)),
+        (('AutoContrast', 0.8, None), ('Solarize', 0.2, 8)), (('Brightness', 0.1, 3), ('Color', 0.7, 0)),
+        (('Solarize', 0.4, 5), ('AutoContrast', 0.9, None)), (('TranslateY', 0.9, 9), ('TranslateY', 0.7, 9)),
+        (('AutoContrast', 0.9, None), ('Solarize', 0.8, 3)), (('Equalize', 0.8, None), ('Invert', 0.1, None)),
+        (('TranslateY', 0.7, 9), ('AutoContrast', 0.9, None))),
+    'svhn': (
+        (('ShearX', 0.9, 4), ('Invert', 0.2, None)), (('ShearY', 0.9, 8), ('Invert', 0.7, None)),
+        (('Equalize', 0.6, None), ('Solarize', 0.6, 6)), (('Invert', 0.9, None), ('Equalize', 0.6, None)),
+        (('Equalize', 0.6, None), ('Rotate', 0.9, 3)), (('ShearX', 0.9, 4), ('AutoContrast', 0.8, None)),
+        (('ShearY', 0.9, 8), ('Invert', 0.4, None)), (('ShearY', 0.9, 5), ('Solarize', 0.2, 6)),
+        (('Invert', 0.9, None), ('AutoContrast', 0.8, None)), (('Equalize', 0.6, None), ('Rotate', 0.9, 3)),
+        (('ShearX', 0.9, 4), ('Solarize', 0.3, 3)), (('ShearY', 0.8, 8), ('Invert', 0.7, None)),
+        (('Equalize', 0.9, None), ('TranslateY', 0.6, 6)), (('Invert', 0.9, None), ('Equalize', 0.6, None)),
+        (('Contrast', 0.3, 3), ('Rotate', 0.8, 4)), (('Invert', 0.8, None), ('TranslateY', 0.0, 2)),
+        (('ShearY', 0.7, 6), ('Solarize', 0.4, 8)), (('Invert', 0.6, None), ('Rotate', 0.8, 4)),
+        (('ShearY', 0.3, 7), ('TranslateX', 0.9, 3)), (('ShearX', 0.1, 6), ('Invert', 0.6, None)),
+        (('Solarize', 0.7, 2), ('TranslateY', 0.6, 7)), (('ShearY', 0.8, 4), ('Invert', 0.8, None)),
+        (('ShearX', 0.7, 9), ('TranslateY', 0.8, 3)), (('ShearY', 0.8, 5), ('AutoContrast', 0.7, None)),
+        (('ShearX', 0.7, 2), ('Invert', 0.1, None))),
+}
+
+
+def aa_magnitudes(bins, h, w):
+    """fp32 [15, bins]: RandAugment's and AutoAugment's magnitude of every op (AA_OPS) and bin on an h x w sample,
+    computed as torchvision computes its tables (torch.linspace, Translate up to 150 / 331 of the side, and the
+    Posterize formula); 0 for the ops without one."""
+    table = torch.zeros(15, bins)
+    for op, (a, b) in {1: (0.0, 0.3), 2: (0.0, 0.3), 3: (0.0, 150.0 / 331.0 * w), 4: (0.0, 150.0 / 331.0 * h),
+                       5: (0.0, 30.0), 6: (0.0, 0.9), 7: (0.0, 0.9), 8: (0.0, 0.9), 9: (0.0, 0.9),
+                       11: (1.0, 0.0)}.items():
+        table[op] = torch.linspace(a, b, bins)
+    table[10] = (8 - (torch.arange(bins) / ((bins - 1) / 4))).round().int()
+    return table.numpy()
+
+
+def ra_ops(rows, num_ops, magnitude, bins, h, w, seed, epoch):
+    """int32 [len(rows), num_ops, 8]: RandAugment(num_ops, magnitude, num_magnitude_bins=bins)'s op rows (ta_ops'
+    format) for every row, slot k's op from row word 65 + 2k and the sign of a signed op's magnitude from 66 + 2k."""
+    mags = aa_magnitudes(bins, h, w)[:, magnitude]
+    hr = _row_hash(rows, seed, epoch)
+    out = np.zeros((len(hr), num_ops, 8), dtype=np.int32)
+    for k in range(num_ops):
+        op = _below(_word(hr, AA_WORD + 2 * k) >> np.uint64(32), 14)
+        neg = _AA_SIGNED[op] & (_u53(hr, AA_WORD + 1 + 2 * k) <= 0.5)
+        out[:, k] = _op_rows(op, np.where(neg, -mags[op], mags[op]).astype(np.float32), h, w)
+    return out
+
+
+def aa_ops(rows, policy, h, w, seed, epoch):
+    """int32 [len(rows), 2, 8]: AutoAugment(policy)'s op rows (ta_ops' format) for every row, the sub-policy from row
+    word 65; op k of the sub-policy runs when u53(word 66 + 2k) <= its probability (else its slot is Identity) and a
+    signed op's magnitude is negated when u53(word 67 + 2k) <= 0.5.  Magnitudes are the 10-bin tables."""
+    subs = AA_POLICIES[policy]
+    mags = aa_magnitudes(10, h, w)
+    hr = _row_hash(rows, seed, epoch)
+    sub = _below(_word(hr, AA_WORD) >> np.uint64(32), len(subs))
+    out = np.zeros((len(hr), 2, 8), dtype=np.int32)
+    for k in range(2):
+        codes = np.asarray([AA_OPS.index(s[k][0]) for s in subs])
+        prob = np.asarray([s[k][1] for s in subs])
+        table = np.asarray([0.0 if s[k][2] is None else mags[AA_OPS.index(s[k][0]), s[k][2]] for s in subs],
+                           dtype=np.float32)
+        run = _u53(hr, AA_WORD + 1 + 2 * k) <= prob[sub]
+        op = np.where(run, codes[sub], 0)
+        mag = np.where(run, table[sub], np.float32(0)).astype(np.float32)
+        neg = _AA_SIGNED[op] & (_u53(hr, AA_WORD + 2 + 2 * k) <= 0.5)
+        out[:, k] = _op_rows(op, np.where(neg, -mag, mag).astype(np.float32), h, w)
     return out
 
 
@@ -842,8 +1001,8 @@ class DeviceResizedImageDataset(_DeviceImageBatches):
     DeviceShardedDataset's.  The kernel takes image and resized sides of at most 32768, resizes at
     most 8x down on each axis and writes rows of at most 1024 values; the constructor refuses anything else.
     augment_params() gives the epoch's indices and boxes.  Batch mixing (random_erase, mixup_alpha, cutmix_alpha, ...)
-    and TrivialAugmentWide (trivial_augment, ta_bins, ta_interpolation) are DeviceImageDataset's, on the
-    size[0] x size[1] output.
+    TrivialAugmentWide (trivial_augment, ta_bins, ta_interpolation) and RandAugment / AutoAugment (auto_augment,
+    ra_num_ops, ra_magnitude, ra_bins) are DeviceImageDataset's, on the size[0] x size[1] output.
     """
 
     def __init__(self, images, labels, batch_size, mean, std, size, scale=(0.08, 1.0), ratio=(3 / 4, 4 / 3),
@@ -851,7 +1010,8 @@ class DeviceResizedImageDataset(_DeviceImageBatches):
                  out_dtype=torch.float32, shuffle=True, even_shards=True, seed=0, aug_seed=None, rank=None,
                  world_size=None, device=None, drop_last=False, mixup_alpha=0.0, cutmix_alpha=0.0, num_classes=None,
                  random_erase=0.0, erase_scale=(0.02, 0.33), erase_ratio=(0.3, 3.3), erase_value=0.0,
-                 trivial_augment=False, ta_bins=31, ta_interpolation='nearest'):
+                 trivial_augment=False, ta_bins=31, ta_interpolation='nearest', auto_augment=None, ra_num_ops=2,
+                 ra_magnitude=9, ra_bins=31):
         H, W, C = _image_hwc(images)
         size = (int(size), int(size)) if isinstance(size, (int, np.integer)) else tuple(int(v) for v in size)
         if len(size) != 2 or min(size) < 1:
@@ -884,7 +1044,7 @@ class DeviceResizedImageDataset(_DeviceImageBatches):
         super().__init__(images, labels, batch_size, mean, std, size, hflip, memory_format, out_dtype, shuffle,
                          even_shards, seed, aug_seed, rank, world_size, device, drop_last, mixup_alpha, cutmix_alpha,
                          num_classes, random_erase, erase_scale, erase_ratio, erase_value, trivial_augment, ta_bins,
-                         ta_interpolation)
+                         ta_interpolation, auto_augment, ra_num_ops, ra_magnitude, ra_bins)
 
     def epoch_table(self):
         """int32 [shard_len(), 5] numpy {top, left, height, width, flipped} of this rank's samples this epoch, in

@@ -536,6 +536,31 @@ int dmlb_image_trivial_augment(const float *src, const int32_t *ops, int64_t bat
                                int bilinear, const dmlb_image_norm *norm, void *out, int out_bf16, int channels_last,
                                void *stream);
 
+/* RandAugment and AutoAugment: a chain of n_ops ops per sample on the float image in [0, 1], then per-channel
+ * normalise, one launch.  dmlb_image_trivial_augment is the one-op case of the same kernel.
+ *   src  : as dmlb_image_trivial_augment's, read only
+ *   ops  : DEVICE int32 [batch][n_ops][8], one dmlb_image_trivial_augment row {op, magnitude, theta0..theta5} per slot
+ *          (util/data.py ra_ops, aa_ops); op codes 0..13 are dmlb_image_trivial_augment's, and
+ *         14 Invert  fl(1 - v), no clamp (torchvision v2's invert of a float image)
+ *   work : DEVICE fp32, min(n_ops - 1, 2) batches of C h w values in src's layout (NULL allowed when n_ops == 1)
+ * Slot k applies its op, with dmlb_image_trivial_augment's rule, to the sample's value after slot k - 1 (src for
+ * k = 0): slots before the last write that value in fp32 into work (alternating between the two work batches when
+ * n_ops >= 3); the last slot normalises into out, out = fl(fl(value - mean[c]) / std[c]).  The statistics of
+ * Contrast, AutoContrast and Equalize are taken over the sample's value before their slot, so Equalize after a Rotate
+ * sees the rotated sample.  An Identity slot reads and writes nothing.  Device data is not checked by the host; the
+ * kernel defines what it does with it: a sample whose src first element is NaN, or with a slot whose op is outside
+ * 0..14 or whose Posterize magnitude is outside (-1, 9), is written all quiet NaN.
+ * Launch: dmlb_image_trivial_augment's clusters; every CTA of a sample's cluster passes a cluster.sync() after each
+ * slot it writes to work, and reads work through L2.
+ * Accepted range (anything else: DMLB_EINVAL, nothing launched): dmlb_image_trivial_augment's, and n_ops in 1..4;
+ * non-NULL work when n_ops >= 2 and batch > 0; work overlapping none of src, ops and out.  DMLB_EALIGN: as
+ * dmlb_image_trivial_augment, and work not aligned to 4 bytes when n_ops >= 2.  Every accepted argument set launches.
+ * Algorithmic bytes/sample, with m the number of slots before the last that are not Identity:
+ * C h w * 4 read + m * C h w * 8 through work + C h w * (4 | 2) written + 32 n_ops B of op rows. */
+int dmlb_image_auto_augment(const float *src, float *work, const int32_t *ops, int32_t n_ops, int64_t batch, int32_t C,
+                            int32_t h, int32_t w, int bilinear, const dmlb_image_norm *norm, void *out, int out_bf16,
+                            int channels_last, void *stream);
+
 #ifdef __cplusplus
 }
 #endif
