@@ -14,7 +14,7 @@ LIB_PATH = Path(__file__).resolve().parent / 'csrc' / 'libdmlb_layers.so'
 
 OK = 0
 EINVAL, EALIGN, ECAPACITY = -10001, -10002, -10003
-ABI_VERSION = 1
+ABI_VERSION = 2
 MAX_BLOCKS = 3
 MAX_C_IN = 4
 MAX_C = 32
@@ -38,6 +38,7 @@ SIGNATURES = {
     'dmll_set_device': (c_int, [c_int]),
     'dmll_layers_launch_count': (c_uint64, []),
     'dmll_cnn_sizes': (c_int, [POINTER(CnnPlan), POINTER(c_int64), POINTER(c_int64)]),
+    'dmll_cnn_cluster_size': (c_int, [POINTER(CnnPlan), c_int64, c_int, POINTER(c_int)]),
     'dmll_cnn_forward_bf16': (c_int, [POINTER(CnnPlan), c_void_p, c_int, c_int64, c_void_p, c_void_p, c_void_p]),
     'dmll_cnn_backward_bf16': (c_int, [POINTER(CnnPlan), c_void_p, c_int64, c_void_p, c_void_p, c_void_p]),
 }

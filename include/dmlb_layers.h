@@ -39,7 +39,7 @@
 extern "C" {
 #endif
 
-#define DMLL_ABI_VERSION 1
+#define DMLL_ABI_VERSION 2
 
 #define DMLL_OK 0
 #define DMLL_EINVAL (-10001)    /* bad argument (null pointer, shape outside the family, batch < 1)      */
@@ -77,6 +77,13 @@ uint64_t dmll_layers_launch_count(void); /* kernels launched through this librar
  * buffer forward writes and backward reads (a multiple of 16).  *n_params: scalars of all weights and biases, i.e. the
  * floats per sample of backward's `partials` workspace. */
 int dmll_cnn_sizes(const dmll_cnn_plan *plan, int64_t *saved_bytes, int64_t *n_params);
+
+/* The cluster size K the launches use for batch n on a GPU of sm_count SMs (pure host function, no GPU needed; it
+ * validates the plan's shapes as dmll_cnn_sizes does).  Each sample runs on a thread-block cluster of K CTAs that split
+ * every block's output channels between them, so a small batch still fills the GPU: K = 1 once n alone fills it,
+ * otherwise the largest K in {2, 4, 8} with n * K within a per-SM constant, never more than the smallest c_out.  The
+ * results are bit-identical for every K. */
+int dmll_cnn_cluster_size(const dmll_cnn_plan *plan, int64_t n, int sm_count, int *cluster);
 
 /* ONE launch.  x: [n][c_in][h][w] fp32 (x_is_bf16 = 0) or bf16 (1).  logits: [n][n_out] bf16.  saved: n * saved_bytes,
  * 16-byte aligned — the bf16 input, every pool's bf16 output and argmax, for backward. */
