@@ -57,6 +57,11 @@ class ImageNorm(Structure):
         return cls(tuple(mean + [0.0] * (4 - len(mean))), tuple(std + [1.0] * (4 - len(std))))
 
 
+class ImageExtent(Structure):
+    """dmlb_image_extent: one image of a packed HWC store (dmlb_image_resample_ragged_u8): byte offset, H and W."""
+    _fields_ = [('offset', c_int64), ('H', c_int32), ('W', c_int32)]
+
+
 class StepMetrics(Structure):
     """dmlb_step_metrics: descriptor of the per-step metric exchange fused into the gradient all-reduce."""
     _fields_ = [('acc', c_void_p), ('cnt', c_void_p), ('desc', c_void_p), ('counter', c_void_p), ('out_ring', c_void_p),
@@ -138,6 +143,9 @@ SIGNATURES = {
     'dmlb_image_resample_u8': (c_int, [c_void_p, c_void_p, c_void_p, c_int64, c_int32, c_int32, c_int32, c_int32, c_int32,
                                        c_int32, c_int32, c_int32, c_int32, POINTER(ImageNorm), c_void_p, c_int, c_int,
                                        c_void_p]),
+    'dmlb_image_resample_ragged_u8': (c_int, [c_void_p, c_int64, c_void_p, c_void_p, c_void_p, c_int64, c_int32, c_int32,
+                                              c_int32, c_int32, c_int32, c_int32, c_int32, POINTER(ImageNorm), c_void_p,
+                                              c_int, c_int, c_void_p]),
     'dmlb_image_mix': (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, POINTER(c_float), c_int64, c_int32, c_int32,
                                c_int32, c_int, c_double, c_int32, c_int32, c_int32, c_int32, c_int32, c_void_p, c_int,
                                c_int, c_void_p, c_void_p]),

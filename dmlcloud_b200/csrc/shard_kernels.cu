@@ -306,8 +306,8 @@ static int dispatch_layout(int out_bf16, int channels_last, const Launch &launch
 
 
 // ---- resampled colour images: box -> antialiased bilinear resize -> window -> flip -> normalise ---------------------
-// (dmlb_image_resample_u8; include/dmlb.h states the rule.)  One CTA job = one band of up to `rows` output rows of one
-// sample.  The CTA builds the sample's column taps (xmin, xsize, weights) for the window's columns and the row taps of
+// (dmlb_image_resample_u8 and, over images of different sizes, dmlb_image_resample_ragged_u8; include/dmlb.h states
+// the rule.)  One CTA job = one band of up to `rows` output rows of one sample.  The CTA builds the sample's column taps (xmin, xsize, weights) for the window's columns and the row taps of
 // the band, runs the horizontal pass over the band's source rows into an fp32 [srows][out_w * C] tile in shared memory,
 // then the vertical pass, written in the output's contiguous order by store_band.  Source bytes are read through
 // L1 (a box row's bytes are read by neighbouring columns' taps) and mapped through a 256-entry fl32(byte) / 255 table.
@@ -321,14 +321,82 @@ constexpr int kResampleBandBytes = 32768;     // target size of a band's tile + 
 constexpr int kResampleCtasPerSm = 4;
 
 struct ResampleArgs {
-    const uint8_t *images;
+    const uint8_t *images;              // [n, H, W, C] images (LaunchGeometry) or the packed store (TableGeometry)
     const long long *idx;
-    const int *boxes;
+    const int *geom;                    // boxes [batch][5] (LaunchGeometry) or geometry rows [batch][9] (TableGeometry)
+    const dmlb_image_extent *extents;   // TableGeometry: one row per image of the store
     void *out;
-    long long batch, sample_bytes;
-    int H, W, C, rh, rw, win_top, win_left, oh, ow;
+    long long batch, sample_bytes;      // sample_bytes: H W C (LaunchGeometry) or the store's bytes (TableGeometry)
+    int H, W, C, rh, rw, win_top, win_left, oh, ow;  // H .. win_left: LaunchGeometry only
     int rows, bands, srows, kx, ky;  // band height, bands per sample, tile rows, column / row tap stride
     float mean[4], std[4];
+};
+
+// One sample's geometry: its image (H x W; where it starts is Geometry::image's), box, flip, resized size and window.
+struct ResampleSample {
+    long long offset;  // TableGeometry: the image's byte offset into the store
+    int H, W, top, left, bh, bw, flip, rh, rw, win_top, win_left;
+};
+
+__host__ __device__ __forceinline__ double resample_dmul(double x, double y) {
+#ifdef __CUDA_ARCH__
+    return __dmul_rn(x, y);
+#else
+    return x * y;
+#endif
+}
+__host__ __device__ __forceinline__ double resample_dadd(double x, double y) {
+#ifdef __CUDA_ARCH__
+    return __dadd_rn(x, y);
+#else
+    return x + y;
+#endif
+}
+
+// Source rows a band of `rows` output rows can read when `in` rows resize to `out`: (rows - 1) scale + 2 support + 1,
+// plus 2 for the fp32 rounding of the tap centres (their error stays below 0.01 row at sides of 32768).  The host
+// plans with it and the kernel admits samples with it, both rounding every operation once, so they agree bit for bit.
+__host__ __device__ __forceinline__ int resample_band_rows(int rows, int in, int out) {
+    const double scale = (double)in / (double)out, support = scale >= 1.0 ? scale : 1.0;
+    return (int)floor(resample_dadd(resample_dadd(resample_dmul(rows - 1, scale), 2.0 * support), 1.0)) + 2;
+}
+
+// Where a sample's geometry comes from.  LaunchGeometry (dmlb_image_resample_u8): the image size, resized size and
+// window are launch constants the host has checked, the box is row i of a [batch][5] table.  TableGeometry
+// (dmlb_image_resample_ragged_u8): the image's extent row and row i of a [batch][9] table, both unchecked device data;
+// a sample whose extent lies outside the store or whose window lies outside its resized image comes back with an empty
+// box (and a 1 x 1 resize), which the kernel's box check turns into a NaN sample.
+struct LaunchGeometry {
+    __device__ __forceinline__ static ResampleSample at(const ResampleArgs &a, long long i) {
+        const int *g = a.geom + 5 * i;
+        return {0, a.H, a.W, g[0], g[1], g[2], g[3], g[4] != 0, a.rh, a.rw, a.win_top, a.win_left};
+    }
+    __device__ __forceinline__ static const uint8_t *image(const ResampleArgs &a, long long i, const ResampleSample &) {
+        return a.images + a.idx[i] * a.sample_bytes;
+    }
+    // The plan is the image's own: every box inside the image fits it.
+    __device__ __forceinline__ static bool fits(const ResampleArgs &, const ResampleSample &, int, int) { return true; }
+};
+
+struct TableGeometry {
+    __device__ __forceinline__ static ResampleSample at(const ResampleArgs &a, long long i) {
+        const int *g = a.geom + 9 * i;
+        const dmlb_image_extent e = a.extents[a.idx[i]];
+        const int rh = g[5], rw = g[6], wt = g[7], wl = g[8];
+        const bool valid = e.H >= 1 && e.W >= 1 && e.H <= kResampleMaxSide && e.W <= kResampleMaxSide &&
+                           e.offset >= 0 && e.offset <= a.sample_bytes - (long long)e.H * e.W * a.C && rh >= 1 &&
+                           rw >= 1 && rh <= kResampleMaxSide && rw <= kResampleMaxSide && wt >= 0 && wl >= 0 &&
+                           wt <= rh - a.oh && wl <= rw - a.ow;
+        if (!valid) return {0, 1, 1, 0, 0, 0, 0, 0, 1, 1, 0, 0};
+        return {e.offset, e.H, e.W, g[0], g[1], g[2], g[3], g[4] != 0, rh, rw, wt, wl};
+    }
+    __device__ __forceinline__ static const uint8_t *image(const ResampleArgs &a, long long, const ResampleSample &s) {
+        return a.images + s.offset;
+    }
+    // The plan is the launch bounds': taps within the strides, a band's source rows within the tile.
+    __device__ __forceinline__ static bool fits(const ResampleArgs &a, const ResampleSample &s, int kx, int ky) {
+        return kx <= a.kx && ky <= a.ky && min(resample_band_rows(a.rows, s.bh, s.rh), s.bh) <= a.srows;
+    }
 };
 
 // One axis of one sample: ATen's antialiased bilinear filter (aten/src/ATen/native/cpu/UpSampleKernel.cpp,
@@ -408,7 +476,12 @@ struct ResampleSmem {
     }
 };
 
-template <bool kBf16, bool kNHWC>
+// A sample is admitted when its box lies inside its image and it fits the launch's plan in every band job
+// (Geometry::fits: taps per output within the strides kx, ky and a band's source rows within the tile, by
+// resample_band_rows at the launch's band height or the box height when that is less).  The test depends on the
+// sample alone, so every band job of a sample decides alike: an admitted sample is resampled whole, any other reads
+// nothing and is quiet NaN whole.
+template <bool kBf16, bool kNHWC, class Geometry>
 __global__ void __launch_bounds__(kResampleThreads) image_resample_u8_kernel(const ResampleArgs a) {
     extern __shared__ float s_dyn[];
     __shared__ float s_lut[256];
@@ -425,24 +498,25 @@ __global__ void __launch_bounds__(kResampleThreads) image_resample_u8_kernel(con
         const long long i = job / a.bands;
         const int y0 = (int)(job - i * a.bands) * a.rows;
         const int nr = min(a.rows, a.oh - y0);
-        const int *box = a.boxes + 5 * i;
-        const int top = box[0], left = box[1], bh = box[2], bw = box[3], flip = box[4] != 0;
-        const int ok = top >= 0 && left >= 0 && bh >= 1 && bw >= 1 && top <= a.H - bh && left <= a.W - bw;
-        const ResampleAxis ax(ok ? bw : 1, a.rw), ay(ok ? bh : 1, a.rh);
-        const int ylo = ay.xmin(a.win_top + y0);
-        const int nsrc = ok ? min(ay.xend(a.win_top + y0 + nr - 1) - ylo, a.srows) : 0;
+        const ResampleSample s = Geometry::at(a, i);
+        int ok = s.top >= 0 && s.left >= 0 && s.bh >= 1 && s.bw >= 1 && s.top <= s.H - s.bh && s.left <= s.W - s.bw;
+        const ResampleAxis ax(ok ? s.bw : 1, s.rw), ay(ok ? s.bh : 1, s.rh);
+        ok = ok && Geometry::fits(a, s, ax.K, ay.K);
+        const int flip = s.flip;
+        const int ylo = ay.xmin(s.win_top + y0);
+        const int nsrc = ok ? ay.xend(s.win_top + y0 + nr - 1) - ylo : 0;
         __syncthreads();  // the previous job's readers are done with the tile and the taps (and the tables are built)
         if (ok) {
             for (int u = threadIdx.x; u < a.ow; u += blockDim.x)
-                ax.taps(a.win_left + u, sm.xmin[u], sm.xsize[u], sm.wx + u * a.kx);
+                ax.taps(s.win_left + u, sm.xmin[u], sm.xsize[u], sm.wx + u * a.kx);
             for (int r = threadIdx.x; r < nr; r += blockDim.x)
-                ay.taps(a.win_top + y0 + r, sm.ymin[r], sm.ysize[r], sm.wy + r * a.ky);
+                ay.taps(s.win_top + y0 + r, sm.ymin[r], sm.ysize[r], sm.wy + r * a.ky);
         }
         __syncthreads();
-        const uint8_t *img = a.images + a.idx[i] * a.sample_bytes + ((long long)(top + ylo) * a.W + left) * a.C;
+        const uint8_t *img = Geometry::image(a, i, s) + ((long long)(s.top + ylo) * s.W + s.left) * a.C;
         for (int t = threadIdx.x; t < nsrc * rowf; t += blockDim.x) {
             const int sr = t / rowf, e = t - sr * rowf, u = e / a.C, c = e - u * a.C;
-            const uint8_t *src = img + ((long long)sr * a.W + sm.xmin[u]) * a.C + c;
+            const uint8_t *src = img + ((long long)sr * s.W + sm.xmin[u]) * a.C + c;
             const float *w = sm.wx + u * a.kx;
             const int n = sm.xsize[u];
             float acc = __fmul_rn(s_lut[__ldg(src)], w[0]);
@@ -470,11 +544,10 @@ static int resample_taps(int in, int out) {
     return (int)std::ceil(scale >= 1.0f ? scale : 1.0f) * 2 + 1;
 }
 
-// Source rows a band of `rows` output rows can read: (rows - 1) scale + 2 support + 1, plus 2 for rounding.
-static int resample_srows(int rows, int H, int rh) {
-    const double scale = (double)H / (double)rh, support = scale >= 1.0 ? scale : 1.0;
-    const int n = (int)std::floor((rows - 1) * scale + 2.0 * support + 1.0) + 2;
-    return n < H ? n : H;
+// Tile rows of a band of `rows` output rows: resample_band_rows, capped by the most rows a box can have.
+static int resample_srows(int rows, int H, int rh, int max_box_h) {
+    const int n = resample_band_rows(rows, H, rh);
+    return n < max_box_h ? n : max_box_h;
 }
 
 constexpr int kResampleMaxTaps = 2 * kResampleMaxScale + 1;
@@ -484,27 +557,47 @@ constexpr size_t kResampleMaxSmem = 4 * ((size_t)kResampleMaxRowElems * (kResamp
 static_assert(kResampleMaxSmem > (size_t)kResampleBandBytes, "a band of one row at the limits exceeds the band target");
 static_assert(kResampleMaxSmem + 2048 <= 227 * 1024, "every accepted launch must fit the opt-in shared memory of sm_90");
 
-static ResamplePlan resample_plan(int H, int W, int C, int rh, int rw, int oh, int ow) {
+// The plan of boxes of up to H x W resized to rh x rw, boxes at most max_box_h rows high (H for one image size; the
+// largest side the kernel takes when the launch bounds only the downscale).
+static ResamplePlan resample_plan(int H, int W, int C, int rh, int rw, int oh, int ow, int max_box_h) {
     ResamplePlan p;
     p.kx = resample_taps(W, rw);
     p.ky = resample_taps(H, rh);
     const size_t row_bytes = (size_t)ow * C * 4;
-    auto band_bytes = [&](int rows) { return 4 * (size_t)rows * (p.ky + 2) + resample_srows(rows, H, rh) * row_bytes; };
+    auto band_bytes = [&](int rows) {
+        return 4 * (size_t)rows * (p.ky + 2) + resample_srows(rows, H, rh, max_box_h) * row_bytes;
+    };
     int rows = 1;
     while (rows < oh && band_bytes(rows + 1) <= (size_t)kResampleBandBytes) ++rows;
     p.bands = (oh + rows - 1) / rows;
     p.rows = (oh + p.bands - 1) / p.bands;
-    p.srows = resample_srows(p.rows, H, rh);
+    p.srows = resample_srows(p.rows, H, rh, max_box_h);
     p.smem = ResampleSmem::bytes(p.srows, ow * C, ow, p.kx, p.rows, p.ky);
     return p;
 }
 
-template <bool kBf16, bool kNHWC>
+template <bool kBf16, bool kNHWC, class Geometry>
 static int launch_resample(int grid, size_t smem, cudaStream_t st, const ResampleArgs &a) {
-    DMLB_CUDA(cudaFuncSetAttribute(image_resample_u8_kernel<kBf16, kNHWC>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                   (int)smem));
-    image_resample_u8_kernel<kBf16, kNHWC><<<grid, kResampleThreads, smem, st>>>(a);
+    DMLB_CUDA(cudaFuncSetAttribute(image_resample_u8_kernel<kBf16, kNHWC, Geometry>,
+                                   cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    image_resample_u8_kernel<kBf16, kNHWC, Geometry><<<grid, kResampleThreads, smem, st>>>(a);
     return launched();
+}
+
+// The launch both resample entries share, on arguments they have checked.  a.images, a.idx, a.geom, a.extents,
+// a.sample_bytes, the LaunchGeometry fields and the norm are the caller's.
+template <class Geometry>
+static int resample_launch(ResampleArgs &a, const ResamplePlan &p, int64_t batch, int32_t C, int32_t out_h,
+                           int32_t out_w, void *out, int out_bf16, int channels_last, void *stream) {
+    a.out = out;
+    a.batch = batch;
+    a.C = C, a.oh = out_h, a.ow = out_w;
+    a.rows = p.rows, a.bands = p.bands, a.srows = p.srows, a.kx = p.kx, a.ky = p.ky;
+    const int grid = band_grid(batch * p.bands, kResampleCtasPerSm);
+    cudaStream_t st = (cudaStream_t)stream;
+    return dispatch_layout(out_bf16, channels_last, [&](auto bf16, auto nhwc) {
+        return launch_resample<decltype(bf16)::value, decltype(nhwc)::value, Geometry>(grid, p.smem, st, a);
+    });
 }
 
 // ---- batch mixing: random erasing -> MixUp or CutMix -> soft targets (dmlb_image_mix) --------------------------------
@@ -1196,21 +1289,43 @@ int dmlb_image_resample_u8(const uint8_t *images, const int64_t *idx, const int3
     if (((uintptr_t)out & (out_bf16 ? 1 : 3)) != 0 || ((uintptr_t)boxes & 3) != 0) return DMLB_EALIGN;
     if (batch == 0) return DMLB_OK;
 
-    const ResamplePlan p = resample_plan(H, W, C, resize_h, resize_w, out_h, out_w);
+    const ResamplePlan p = resample_plan(H, W, C, resize_h, resize_w, out_h, out_w, H);
     a.images = images;
     a.idx = (const long long *)idx;
-    a.boxes = boxes;
-    a.out = out;
-    a.batch = batch;
+    a.geom = boxes;
+    a.extents = nullptr;
     a.sample_bytes = (long long)H * W * C;
-    a.H = H, a.W = W, a.C = C, a.rh = resize_h, a.rw = resize_w, a.win_top = win_top, a.win_left = win_left;
-    a.oh = out_h, a.ow = out_w;
-    a.rows = p.rows, a.bands = p.bands, a.srows = p.srows, a.kx = p.kx, a.ky = p.ky;
-    const int grid = band_grid(batch * p.bands, kResampleCtasPerSm);
-    cudaStream_t st = (cudaStream_t)stream;
-    return dispatch_layout(out_bf16, channels_last, [&](auto bf16, auto nhwc) {
-        return launch_resample<decltype(bf16)::value, decltype(nhwc)::value>(grid, p.smem, st, a);
-    });
+    a.H = H, a.W = W, a.rh = resize_h, a.rw = resize_w, a.win_top = win_top, a.win_left = win_left;
+    return resample_launch<LaunchGeometry>(a, p, batch, C, out_h, out_w, out, out_bf16, channels_last, stream);
+}
+
+int dmlb_image_resample_ragged_u8(const uint8_t *store, int64_t store_bytes, const dmlb_image_extent *extents,
+                                  const int64_t *idx, const int32_t *geom, int64_t batch, int32_t C, int32_t bound_h,
+                                  int32_t bound_rh, int32_t bound_w, int32_t bound_rw, int32_t out_h, int32_t out_w,
+                                  const dmlb_image_norm *norm, void *out, int out_bf16, int channels_last,
+                                  void *stream) {
+    if (batch < 0 || store_bytes < 0 || !norm || C < 1 || C > 4) return DMLB_EINVAL;
+    for (int32_t side : {bound_h, bound_rh, bound_w, bound_rw, out_h, out_w})
+        if (side < 1 || side > kResampleMaxSide) return DMLB_EINVAL;
+    if ((long long)bound_h > (long long)kResampleMaxScale * bound_rh ||
+        (long long)bound_w > (long long)kResampleMaxScale * bound_rw)
+        return DMLB_EINVAL;
+    if ((long long)out_w * C > kResampleMaxRowElems) return DMLB_EINVAL;
+    ResampleArgs a;
+    if (!pack_norm(norm, C, a.mean, a.std)) return DMLB_EINVAL;
+    if (batch > 0 && (!store || !extents || !idx || !geom || !out)) return DMLB_EINVAL;
+    if (((uintptr_t)out & (out_bf16 ? 1 : 3)) != 0 || ((uintptr_t)geom & 3) != 0 || ((uintptr_t)extents & 7) != 0)
+        return DMLB_EALIGN;
+    if (batch == 0) return DMLB_OK;
+
+    const ResamplePlan p = resample_plan(bound_h, bound_w, C, bound_rh, bound_rw, out_h, out_w, kResampleMaxSide);
+    a.images = store;
+    a.idx = (const long long *)idx;
+    a.geom = geom;
+    a.extents = extents;
+    a.sample_bytes = store_bytes;
+    a.H = a.W = a.rh = a.rw = a.win_top = a.win_left = 0;
+    return resample_launch<TableGeometry>(a, p, batch, C, out_h, out_w, out, out_bf16, channels_last, stream);
 }
 
 int dmlb_image_mix(const float *src, const int64_t *idx, const int64_t *labels, const int32_t *erase, const float *fill,

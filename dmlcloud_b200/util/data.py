@@ -239,7 +239,7 @@ class DeviceShardedDataset:
         self.images = images.to(self.device).contiguous()
         self.labels = labels.to(self.device, dtype=torch.int64).contiguous()
         self.item_shape = tuple(images.shape[1:])
-        self.row_elems = int(np.prod(self.item_shape)) if self.item_shape else 1
+        self.row_elems = None if None in self.item_shape else int(np.prod(self.item_shape))
         self.batch_size = batch_size
         self.mean, self.std = float(mean), float(std)
         self.shuffle, self.even_shards, self.seed = shuffle, even_shards, seed
@@ -306,6 +306,73 @@ def _image_hwc(images):
     if images.dim() != 4 or not 1 <= images.shape[3] <= 4:
         raise ValueError('images must be uint8 [N, H, W, C] with 1 <= C <= 4')
     return tuple(int(v) for v in images.shape[1:])
+
+
+class PackedImages:
+    """uint8 HWC images of different sizes and one channel count C, packed back to back into one byte store: image i
+    is store[offsets[i] : offsets[i] + H_i W_i C] (pack_images).  extents is the int32 [N, 4] table of
+    dmlb_image_extent rows {offset (low, high word), H, W}; offsets (int64 [N]) and sizes (int64 [N, 2] {H, W}) are
+    the host's copies.  It stands where a [N, H, W, C] tensor stands in the datasets: shape is (N, None, None, C) and
+    to(device) copies the store and the table once each."""
+    dtype = torch.uint8
+
+    def __init__(self, store, extents, offsets, sizes, C):
+        self.store, self.extents, self.offsets, self.sizes = store, extents, offsets, sizes
+        self.shape = (len(sizes), None, None, C)
+
+    def to(self, device):
+        return PackedImages(self.store.to(device), self.extents.to(device), self.offsets, self.sizes, self.shape[3])
+
+    def contiguous(self):
+        return self
+
+    def image(self, i):
+        """Image i as a uint8 [H, W, C] view of the store."""
+        (H, W), off, C = (int(v) for v in self.sizes[i]), int(self.offsets[i]), self.shape[3]
+        return self.store[off:off + H * W * C].view(H, W, C)
+
+
+def pack_images(images):
+    """PackedImages of a sequence of uint8 [H, W, C] arrays or tensors (any H, W >= 1; one C in 1..4), packed on the
+    host in sequence order.  Refuses an empty sequence, an image that is not uint8 [H, W, C] with H, W >= 1 and C in
+    1..4, and mixed C, naming the first offending image."""
+    arrays = []
+    for i, img in enumerate(images):
+        a = img.detach().cpu().numpy() if isinstance(img, torch.Tensor) else np.asarray(img)
+        if a.dtype != np.uint8 or a.ndim != 3 or min(a.shape[:2]) < 1 or not 1 <= a.shape[2] <= 4:
+            raise ValueError(f'image {i} must be uint8 [H, W, C] with H, W >= 1 and 1 <= C <= 4, got {a.dtype} '
+                             f'{list(a.shape)}')
+        if arrays and a.shape[2] != arrays[0].shape[2]:
+            raise ValueError(f'image {i} ({a.shape[0]}x{a.shape[1]}) has {a.shape[2]} channels, image 0 has '
+                             f'{arrays[0].shape[2]}: one dataset takes one channel count')
+        arrays.append(a)
+    if not arrays:
+        raise ValueError('images is empty')
+    sizes = np.asarray([a.shape[:2] for a in arrays], dtype=np.int64)
+    nbytes = np.asarray([a.size for a in arrays], dtype=np.int64)
+    offsets = np.concatenate([[0], np.cumsum(nbytes)[:-1]]).astype(np.int64)
+    store = torch.empty(int(nbytes.sum()), dtype=torch.uint8)
+    flat = store.numpy()
+    for a, off, n in zip(arrays, offsets, nbytes):
+        flat[off:off + n] = a.reshape(-1)
+    extents = np.empty((len(arrays), 4), dtype=np.int32)
+    extents[:, :2] = offsets.view(np.int32).reshape(-1, 2)
+    extents[:, 2:] = sizes
+    return PackedImages(store, torch.from_numpy(extents), offsets, sizes, int(arrays[0].shape[2]))
+
+
+class RaggedTable:
+    """The geometry rows of a ragged epoch: `rows` on the device (what the kernel reads) and `host`, their numpy copy
+    (what each launch takes its bounds from, with no device sync).  Slicing slices both."""
+
+    def __init__(self, rows, host):
+        self.rows, self.host = rows, host
+
+    def __getitem__(self, s):
+        return RaggedTable(self.rows[s], self.host[s])
+
+    def __len__(self):
+        return len(self.host)
 
 
 class _DeviceImageBatches(DeviceShardedDataset):
@@ -672,16 +739,16 @@ def crop_windows(rows, H, W, out_h, out_w, pad, random_crop, hflip, seed, epoch)
 def resized_crop_boxes(rows, H, W, scale, ratio, seed, epoch, hflip):
     """int32 [len(rows), 5] {top, left, height, width, flipped}: torchvision RandomResizedCrop.get_params for every
     row, drawn from row words 2..31 (and 1 for the flip); w and h round halves to even, and after 10 failed attempts
-    the box is torchvision's central fallback.  fp64 numpy, vectorised over the rows."""
+    the box is torchvision's central fallback.  H and W are the image size of every row (ints) or of each row (arrays
+    of len(rows)); a row's box depends only on its own size.  fp64 numpy, vectorised over the rows."""
     h = _row_hash(rows, seed, epoch)
+    H = np.broadcast_to(np.asarray(H, dtype=np.int64), h.shape)
+    W = np.broadcast_to(np.asarray(W, dtype=np.int64), h.shape)
     in_ratio = W / H
-    if in_ratio < min(ratio):
-        fw, fh = W, int(round(W / min(ratio)))
-    elif in_ratio > max(ratio):
-        fh, fw = H, int(round(H * max(ratio)))
-    else:
-        fw, fh = W, H
-    box = np.tile(np.asarray([(H - fh) // 2, (W - fw) // 2, fh, fw], dtype=np.int64), (len(h), 1))
+    narrow, wide = in_ratio < min(ratio), in_ratio > max(ratio)
+    fw = np.where(wide, np.rint(H * max(ratio)).astype(np.int64), W)
+    fh = np.where(narrow, np.rint(W / min(ratio)).astype(np.int64), H)
+    box = np.stack([(H - fh) // 2, (W - fw) // 2, fh, fw], axis=-1)
     done = np.zeros(len(h), dtype=bool)
     lr0, lr1 = np.log(ratio[0]), np.log(ratio[1])
     for a in range(10):
@@ -692,10 +759,29 @@ def resized_crop_boxes(rows, H, W, scale, ratio, seed, epoch, hflip):
         ok = ~done & (w > 0) & (w <= W) & (hh > 0) & (hh <= H)
         if ok.any():
             off = _word(h[ok], 4 + 3 * a)
-            box[ok] = np.stack([_below(off & np.uint64(0xFFFFFFFF), H - hh[ok] + 1),
-                                _below(off >> np.uint64(32), W - w[ok] + 1), hh[ok], w[ok]], axis=-1)
+            box[ok] = np.stack([_below(off & np.uint64(0xFFFFFFFF), H[ok] - hh[ok] + 1),
+                                _below(off >> np.uint64(32), W[ok] - w[ok] + 1), hh[ok], w[ok]], axis=-1)
             done |= ok
     return np.concatenate([box, _flips(h, hflip)[:, None]], axis=1).astype(np.int32)
+
+
+def resize_windows(H, W, S, size):
+    """int64 [n, 4] {resize_h, resize_w, win_top, win_left} of images of H x W (int arrays): torchvision Resize(S) (the
+    short side becomes S, the long side int(S * long / short)) and the offsets of CenterCrop(size) in the result
+    (round((resized - size) / 2), halves to even)."""
+    H, W = np.asarray(H, dtype=np.int64), np.asarray(W, dtype=np.int64)
+    long = (S * np.maximum(H, W) / np.minimum(H, W)).astype(np.int64)
+    rh, rw = np.where(W <= H, long, S), np.where(W <= H, S, long)
+    return np.stack([rh, rw, np.rint((rh - size[0]) / 2.0).astype(np.int64),
+                     np.rint((rw - size[1]) / 2.0).astype(np.int64)], axis=-1)
+
+
+def ragged_bounds(geom):
+    """(bound_h, bound_rh, bound_w, bound_rw) of int32 [n >= 1, 9] geometry rows: on each axis the box and resized
+    sides of the row with the largest downscale, the launch bounds of dmlb_image_resample_ragged_u8."""
+    g = np.asarray(geom, dtype=np.int64)
+    i, j = int(np.argmax(g[:, 2] / g[:, 5])), int(np.argmax(g[:, 3] / g[:, 6]))
+    return int(g[i, 2]), int(g[i, 5]), int(g[j, 3]), int(g[j, 6])
 
 
 ERASE_WORD = 32  # the erase words of a row, 32..62, follow the crop and flip words (0..31)
@@ -991,7 +1077,9 @@ class DeviceResizedImageDataset(_DeviceImageBatches):
     """Device-resident colour-image dataset with the ImageNet recipes (SURVEY §8f-1), one resampling launch per batch
     (dmlb_image_resample_u8) plus the label gather.
 
-    images: uint8 [N, H, W, C] (HWC, C <= 4), labels: int64 [N].  size: int or (h, w) of the output.
+    images: uint8 [N, H, W, C] (HWC, C <= 4), or a sequence of N uint8 [H, W, C] arrays or tensors of any sizes and
+    one C (an FFCV-style store of images decoded once at their own size); labels: int64 [N].  size: int or (h, w) of
+    the output.
       random=True  (training): torchvision RandomResizedCrop(size, scale, ratio) -> RandomHorizontalFlip (if hflip)
                    -> Normalize; the boxes of an epoch are sampled on the host (resized_crop_boxes) and uploaded once.
       random=False (validation): Resize(resize) -> CenterCrop(size) -> Normalize (flipped when hflip, like training).
@@ -1003,6 +1091,17 @@ class DeviceResizedImageDataset(_DeviceImageBatches):
     augment_params() gives the epoch's indices and boxes.  Batch mixing (random_erase, mixup_alpha, cutmix_alpha, ...)
     TrivialAugmentWide (trivial_augment, ta_bins, ta_interpolation) and RandAugment / AutoAugment (auto_augment,
     ra_num_ops, ra_magnitude, ra_bins) are DeviceImageDataset's, on the size[0] x size[1] output.
+
+    Images of different sizes are packed on the host into one byte store with an extent table (pack_images,
+    PackedImages) and copied to the device once.  Every sample is what torchvision does to its own image: training
+    draws its RandomResizedCrop box at its own size (resized_crop_boxes with per-row sizes), validation takes
+    Resize(resize) and the CenterCrop offsets of its own image (resize_windows).  Each batch is one
+    dmlb_image_resample_ragged_u8 launch, planned for the largest downscale in the batch (ragged_bounds, from the
+    host's copy of the table); everything after it is as above.  epoch_table() rows then have 9 columns and
+    augment_params() gives a RaggedTable.  The constructor refuses an empty sequence, an image that is not uint8
+    [H, W, C], mixed C, an image or resized side above 32768, more than an 8x downscale and, in validation, a size
+    larger than an image's resized size, naming the first image at fault.  A list of equal-size images gives the
+    batches of their [N, H, W, C] tensor, bit for bit.
     """
 
     def __init__(self, images, labels, batch_size, mean, std, size, scale=(0.08, 1.0), ratio=(3 / 4, 4 / 3),
@@ -1012,7 +1111,12 @@ class DeviceResizedImageDataset(_DeviceImageBatches):
                  random_erase=0.0, erase_scale=(0.02, 0.33), erase_ratio=(0.3, 3.3), erase_value=0.0,
                  trivial_augment=False, ta_bins=31, ta_interpolation='nearest', auto_augment=None, ra_num_ops=2,
                  ra_magnitude=9, ra_bins=31):
-        H, W, C = _image_hwc(images)
+        self._ragged = not isinstance(images, torch.Tensor)
+        if self._ragged:
+            images = pack_images(images)
+            C = images.shape[3]
+        else:
+            H, W, C = _image_hwc(images)
         size = (int(size), int(size)) if isinstance(size, (int, np.integer)) else tuple(int(v) for v in size)
         if len(size) != 2 or min(size) < 1:
             raise ValueError(f'size must be a positive int or (h, w), got {size}')
@@ -1029,16 +1133,20 @@ class DeviceResizedImageDataset(_DeviceImageBatches):
         else:
             if resize is None or int(resize) < 1:
                 raise ValueError('validation (random=False) needs resize, the short side S of Resize(S)')
-            short, long = min(H, W), max(H, W)
-            S, L = int(resize), int(int(resize) * long / short)
-            self.resized = (L, S) if W <= H else (S, L)
-            if size[0] > self.resized[0] or size[1] > self.resized[1]:
-                raise ValueError(f'size {size} is larger than the resized image {self.resized}')
-            self.window = tuple(int(round((r - s) / 2.0)) for r, s in zip(self.resized, size))
-        if max(H, W, *self.resized) > 32768:
-            raise ValueError(f'{H}x{W} images resized to {self.resized}: the kernel takes sides of at most 32768')
-        if H > 8 * self.resized[0] or W > 8 * self.resized[1]:
-            raise ValueError(f'{H}x{W} images resized to {self.resized} is more than an 8x downscale')
+        if self._ragged:
+            self._check_ragged(images, size, resize)
+        else:
+            if not self.random:
+                short, long = min(H, W), max(H, W)
+                S, L = int(resize), int(int(resize) * long / short)
+                self.resized = (L, S) if W <= H else (S, L)
+                if size[0] > self.resized[0] or size[1] > self.resized[1]:
+                    raise ValueError(f'size {size} is larger than the resized image {self.resized}')
+                self.window = tuple(int(round((r - s) / 2.0)) for r, s in zip(self.resized, size))
+            if max(H, W, *self.resized) > 32768:
+                raise ValueError(f'{H}x{W} images resized to {self.resized}: the kernel takes sides of at most 32768')
+            if H > 8 * self.resized[0] or W > 8 * self.resized[1]:
+                raise ValueError(f'{H}x{W} images resized to {self.resized} is more than an 8x downscale')
         if size[1] * C > 1024:
             raise ValueError(f'size[1] * C = {size[1] * C} is above the 1024 values per output row the kernel takes')
         super().__init__(images, labels, batch_size, mean, std, size, hflip, memory_format, out_dtype, shuffle,
@@ -1046,20 +1154,69 @@ class DeviceResizedImageDataset(_DeviceImageBatches):
                          num_classes, random_erase, erase_scale, erase_ratio, erase_value, trivial_augment, ta_bins,
                          ta_interpolation, auto_augment, ra_num_ops, ra_magnitude, ra_bins)
 
+    def _check_ragged(self, images, size, resize):
+        """The geometry of every image of the PackedImages `images` (self._geometry: int64 [N, 4] {resize_h, resize_w,
+        win_top, win_left}), refusing the first image the kernel cannot resample."""
+        Hs, Ws = images.sizes[:, 0], images.sizes[:, 1]
+        if self.random:
+            geo = np.tile(np.asarray([size[0], size[1], 0, 0], dtype=np.int64), (len(Hs), 1))
+        else:
+            geo = resize_windows(Hs, Ws, int(resize), size)
+            self.resized = self.window = None  # per image: self._geometry
+        rh, rw = geo[:, 0], geo[:, 1]
+
+        def refuse(bad, why):
+            if bad.any():
+                i = int(np.argmax(bad))
+                raise ValueError(f'image {i} ({Hs[i]}x{Ws[i]}) resized to ({rh[i]}, {rw[i]}): {why}')
+
+        refuse(np.maximum(Hs, Ws) > 32768, 'the kernel takes image sides of at most 32768')
+        refuse(np.maximum(rh, rw) > 32768, 'the kernel takes resized sides of at most 32768')
+        refuse((Hs > 8 * rh) | (Ws > 8 * rw), 'more than an 8x downscale')
+        refuse((rh < size[0]) | (rw < size[1]), f'size {size} is larger than the resized image')
+        self._geometry = geo
+
     def epoch_table(self):
         """int32 [shard_len(), 5] numpy {top, left, height, width, flipped} of this rank's samples this epoch, in
-        iteration order: resized_crop_boxes, or the whole image with the same flips in validation."""
-        H, W, _ = self.item_shape
+        iteration order: resized_crop_boxes, or the whole image with the same flips in validation.  For images of
+        different sizes, int32 [shard_len(), 9]: each row followed by its image's {resize_h, resize_w, win_top,
+        win_left}."""
         rows = self._shard_rows()
+        if self._ragged:
+            Hs, Ws = self.images.sizes[rows, 0], self.images.sizes[rows, 1]
+            if self.random:
+                boxes = resized_crop_boxes(rows, Hs, Ws, self.scale, self.ratio, self.aug_seed, self.epoch,
+                                           self.hflip)
+            else:
+                boxes = np.zeros((len(rows), 5), dtype=np.int64)
+                boxes[:, 2], boxes[:, 3] = Hs, Ws
+                boxes[:, 4] = _flips(_row_hash(rows, self.aug_seed, self.epoch), self.hflip)
+            return np.concatenate([boxes, self._geometry[rows]], axis=1).astype(np.int32)
+        H, W, _ = self.item_shape
         if self.random:
             return resized_crop_boxes(rows, H, W, self.scale, self.ratio, self.aug_seed, self.epoch, self.hflip)
         boxes = np.tile(np.asarray([0, 0, H, W, 0], dtype=np.int32), (len(rows), 1))
         boxes[:, 4] = _flips(_row_hash(rows, self.aug_seed, self.epoch), self.hflip)
         return boxes
 
+    def augment_params(self):
+        """(indices, table): this rank's dataset indices for the current epoch in iteration order and the device copy
+        of epoch_table(); for images of different sizes, a RaggedTable holding it with its host copy."""
+        if not self._ragged:
+            return super().augment_params()
+        table = self.epoch_table()
+        return self.epoch_indices(), RaggedTable(torch.from_numpy(table).to(self.device), table)
+
     def _launch(self, view, boxes, x, norm):
         N = self._N
         H, W, C = self.item_shape
+        if self._ragged:  # boxes: the batch's RaggedTable rows; the launch bounds come from their host copy
+            N.check(N.cuda_lib(self.device.index).dmlb_image_resample_ragged_u8(
+                self.images.store.data_ptr(), self.images.store.numel(), self.images.extents.data_ptr(),
+                view.data_ptr(), boxes.rows.data_ptr(), view.numel(), C, *ragged_bounds(boxes.host), *self.crop,
+                norm, x.data_ptr(), int(x.dtype == torch.bfloat16), int(self.memory_format == torch.channels_last),
+                N.stream_ptr()), 'image_resample_ragged_u8')
+            return
         N.check(N.cuda_lib(self.device.index).dmlb_image_resample_u8(
             self.images.data_ptr(), view.data_ptr(), boxes.data_ptr(), view.numel(), H, W, C, *self.resized,
             *self.window, *self.crop, norm, x.data_ptr(), int(x.dtype == torch.bfloat16),

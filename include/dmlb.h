@@ -451,6 +451,41 @@ int dmlb_image_resample_u8(const uint8_t *images, const int64_t *idx, const int3
                            int32_t out_h, int32_t out_w, const dmlb_image_norm *norm, void *out, int out_bf16,
                            int channels_last, void *stream);
 
+/* Resampled colour-image batch from images of different sizes: dmlb_image_resample_u8's rule, with every sample's
+ * image, box, resized size and window taken from two device tables instead of launch constants.
+ *   store   : uint8 bytes holding every image packed as HWC (C channels each); store_bytes of them
+ *   extents : DEVICE dmlb_image_extent [n], one row per image: its byte offset into store (64-bit: stores beyond 4 GiB
+ *             work), its H and W; row i of the batch is image idx[i]
+ *   geom    : DEVICE int32 [batch][9] {top, left, height, width, flipped, resize_h, resize_w, win_top, win_left}
+ *   out     : logical [batch, C, out_h, out_w], NCHW (channels_last == 0) or NHWC in memory, fp32 or bf16 (RNE)
+ * Sample i: the box of image idx[i] is resized to resize_h x resize_w, the out_h x out_w window at (win_top, win_left)
+ * is taken and flipped, and every value is dmlb_image_resample_u8's for that image and geometry, bit for bit.  Values do
+ * not depend on the bounds, the batch or a sample's place in it: equal-size images give dmlb_image_resample_u8's bits.
+ * bound_h / bound_rh and bound_w / bound_rw bound every sample's downscale (height / resize_h <= bound_h / bound_rh and
+ * width / resize_w <= bound_w / bound_rw); the launch is planned for them as dmlb_image_resample_u8 plans an image of
+ * bound_h x bound_w resized to bound_rh x bound_rw (the host takes them from the table it uploads).
+ * Accepted range (anything else: DMLB_EINVAL, nothing launched): C in 1..4; bound_h, bound_rh, bound_w, bound_rw, out_h,
+ * out_w in 1..32768; bound_h <= 8 bound_rh and bound_w <= 8 bound_rw; out_w * C <= 1024; store_bytes >= 0;
+ * std[c] != 0 for c < C; non-NULL norm, and store / extents / idx / geom / out when batch > 0.  DMLB_EALIGN: out not
+ * aligned to its element, geom not to 4 bytes or extents not to 8.  Every accepted argument set launches (shared memory
+ * as dmlb_image_resample_u8).  The tables live in device memory and are not checked by the host; the kernel admits
+ * sample i only when its extent has H, W in 1..32768 and lies inside store, its box is inside the image, resize_h and
+ * resize_w lie in 1..32768, its window is inside the resized image, and its taps per output and a band's source rows fit
+ * the plan of the bounds (which every sample within the bounds does).  Any other sample reads nothing and writes quiet
+ * NaN over the whole sample.  Any store alignment works.
+ * Algorithmic bytes/sample: box bytes read (at most) + out_h * out_w * C * (4 | 2) written + 36 B of geometry + 16 B of
+ * extent. */
+typedef struct {
+    int64_t offset;
+    int32_t H;
+    int32_t W;
+} dmlb_image_extent;
+int dmlb_image_resample_ragged_u8(const uint8_t *store, int64_t store_bytes, const dmlb_image_extent *extents,
+                                  const int64_t *idx, const int32_t *geom, int64_t batch, int32_t C, int32_t bound_h,
+                                  int32_t bound_rh, int32_t bound_w, int32_t bound_rw, int32_t out_h, int32_t out_w,
+                                  const dmlb_image_norm *norm, void *out, int out_bf16, int channels_last,
+                                  void *stream);
+
 /* Batch mixing: random erasing per sample, then MixUp or CutMix over the batch, then the targets, one launch.
  * torchvision v2's RandomErasing(value=fill) on every sample, then MixUp or CutMix (pairing sample i with i - 1 mod
  * batch, torchvision's roll(1, 0)), and their one_hot targets mixed by _BaseMixUpCutMix._mixup_label.
